@@ -776,9 +776,6 @@ __global__ void __launch_bounds__(VM_NT, 4) radix_rows_kernel(const VMProgramHea
   }
 }
 
-__global__ void rg_digit_kernel(const uint32_t* __restrict__ h, int64_t n, int shift, uint32_t mask, int32_t* __restrict__ pid) {
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) pid[i] = (int32_t)((h[i] >> shift) & mask);
-}
 // rows are sorted by q = h & (P - 1): off[q] = first row of partition q, off[P] = n
 __global__ void rg_offsets_kernel(const uint32_t* __restrict__ h, int64_t n, uint32_t pmask, int32_t* __restrict__ off) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
@@ -996,6 +993,237 @@ __global__ void __launch_bounds__(RG_NT, 1) radix_agg_kernel(const __grid_consta
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// Specialised radix aggregation: the shape of TPC-H q3 and of most high-cardinality group-bys — NOT NULL keys in one or two
+// packed words, SUM / COUNT over NOT NULL integer or decimal values.  Everything the generic kernel reads from the plan per row
+// is a template parameter here, and every accumulator is kept as 32-bit words updated by NATIVE shared-memory atomics (a 64-bit
+// shared-memory atomicAdd is a compare-and-swap loop on this architecture).
+//
+// A value is split into 32-bit pieces x0 .. x{K-1} (K = 2 for 64-bit values, 4 for 128-bit ones; the top piece is signed) and
+// added piece by piece with a ripple carry: piece j plus the carry out of piece j - 1 is added to word j by atomicAdd, and the
+// word's wrap is read off the returned old value.  The signed top piece carries -1 / 0 / +1 into one extension word.  Zero
+// addends are skipped, so a small positive value (every q3 row) costs ONE atomic.  Whatever the order of the atomics, word j
+// ends as the sum's bits [32j, 32j + 32) and the extension as the sign-extended rest, so the flush rebuilds the exact two's-
+// complement sum the generic kernel's 64-bit limbs hold: 1 limb (wrapping INT64 sum: no extension word), 2 limbs (64-bit
+// decimal), 3 limbs (128-bit decimal).
+enum : uint32_t { RF_COUNT = 1, RF_SUM64 = 2, RF_SUMDEC64 = 3, RF_SUMDEC128 = 4 };
+// aggregate k of a signature: kind in bits [8k, 8k + 4), value slot in bits [8k + 4, 8k + 8)
+constexpr uint32_t rf_agg(uint32_t kind, uint32_t slot, int k) { return (kind | slot << 4) << (8 * k); }
+constexpr uint32_t rf_kind(uint32_t sig, int k) { return (sig >> (8 * k)) & 15u; }
+constexpr int rf_slot(uint32_t sig, int k) { return (int)((sig >> (8 * k + 4)) & 15u); }
+constexpr int rf_words(uint32_t kind) { return kind == RF_COUNT ? 1 : kind == RF_SUM64 ? 2 : kind == RF_SUMDEC64 ? 3 : 5; }
+constexpr int rf_limbs(uint32_t kind) { return kind == RF_SUMDEC64 ? 2 : kind == RF_SUMDEC128 ? 3 : 1; }
+template <uint32_t SIG, int NA> constexpr int rf_word_off(int k) { int o = 0; for (int j = 0; j < k; j++) o += rf_words(rf_kind(SIG, j)); return o; }
+template <uint32_t SIG, int NA> constexpr int rf_limb_off(int k) { int o = 0; for (int j = 0; j < k; j++) o += rf_limbs(rf_kind(SIG, j)); return o; }
+// the width of value slot s: 16 bytes when a 128-bit decimal sum reads it
+template <uint32_t SIG, int NA> constexpr int rf_vwidth(int s) {
+  for (int k = 0; k < NA; k++) if (rf_slot(SIG, k) == s && rf_kind(SIG, k) == RF_SUMDEC128) return 16;
+  return 8;
+}
+constexpr int RF_NT = 512;
+constexpr int RF_CHUNK = 512;   // rows per staged chunk: one per thread
+constexpr int RF_NBUF = 3;      // stage buffers: the previous chunk's rows stay readable while the next one is in flight
+// one stage buffer: k0 | k1 | v[0..NV), RF_CHUNK rows each + 16 bytes of slack for the rounded-up copies
+template <int NK, int NV, int NA, uint32_t SIG> constexpr int rf_soff_v(int s) {
+  int o = (RF_CHUNK * 8 + 16) * NK;
+  for (int q = 0; q < s; q++) o += RF_CHUNK * rf_vwidth<SIG, NA>(q) + 16;
+  return o;
+}
+template <int NK, int NV, int NA, uint32_t SIG> constexpr int rf_stage_bytes() { return (rf_soff_v<NK, NV, NA, SIG>(NV) + 127) & ~127; }
+
+template <int K>   // words of the value (2: 64-bit, 4: 128-bit); EXT: keep the extension word (exact sums)
+__device__ __forceinline__ void rf_add(uint32_t* w, int C, int slot, const uint32_t (&x)[K], bool ext_word) {
+  uint32_t c = 0;
+#pragma unroll
+  for (int j = 0; j < K - 1; j++) {
+    const uint32_t a = x[j] + c;
+    uint32_t cj = a < c;                       // x[j] + carry wrapped by itself (x[j] = 0xffffffff, carry 1)
+    if (a) { const uint32_t old = atomicAdd(&w[j * C + slot], a); cj += old + a < old; }
+    c = cj;
+  }
+  const int64_t t = (int64_t)(int32_t)x[K - 1] + c;   // signed top piece plus carry: [-2^31, 2^31]
+  const uint32_t a = (uint32_t)t;
+  int32_t up = (int32_t)(t >> 32);                   // -1 or 0
+  if (a) { const uint32_t old = atomicAdd(&w[(K - 1) * C + slot], a); up += old + a < old; }
+  if (ext_word && up) atomicAdd(&w[K * C + slot], (uint32_t)up);
+}
+
+template <int NK, int NV, int NA, uint32_t SIG>
+__global__ void __launch_bounds__(RF_NT, 1) radix_agg_fixed_kernel(const __grid_constant__ RGAgg a) {
+  constexpr int CH = RF_CHUNK;
+  constexpr int NW = rf_word_off<SIG, NA>(NA);     // accumulator words per slot
+  constexpr int LIMBS = NA ? rf_limb_off<SIG, NA>(NA) : 1;
+  constexpr int SOFF_K1 = CH * 8 + 16;
+  constexpr int SBYTES = rf_stage_bytes<NK, NV, NA, SIG>();
+  auto soff_v = [](int s) { return rf_soff_v<NK, NV, NA, SIG>(s); };
+  extern __shared__ __align__(128) char rg_dyn[];
+  __shared__ __align__(8) uint64_t s_bar[RF_NBUF];
+  __shared__ uint32_t s_nused, s_nflush;
+  __shared__ unsigned long long s_obase;
+  const int C = a.C;
+  // table: packed keys, 32-bit accumulator words [word][C], state (0 = empty, else 1 + the claiming row's position in the
+  // stage buffers [| RG_READY once the key is published]), log of the claimed slots; then the stage buffers
+  uint64_t* t_k0 = reinterpret_cast<uint64_t*>(rg_dyn);
+  uint64_t* t_k1 = t_k0 + C;
+  uint32_t* t_w = reinterpret_cast<uint32_t*>(t_k1 + (NK == 2 ? C : 0));
+  uint32_t* t_state = t_w + (size_t)NW * C;
+  uint16_t* t_used = reinterpret_cast<uint16_t*>(t_state + C);
+  char* stage0 = reinterpret_cast<char*>(((uintptr_t)(t_used + C) + 127) & ~(uintptr_t)127);
+  for (int s = threadIdx.x; s < C; s += RF_NT) {
+    t_state[s] = 0;
+#pragma unroll
+    for (int j = 0; j < NW; j++) t_w[j * C + s] = 0;
+  }
+  const int pA = (int)((int64_t)a.P * blockIdx.x / gridDim.x), pB = (int)((int64_t)a.P * (blockIdx.x + 1) / gridDim.x);
+  const int64_t r_lo = a.off[pA], r_hi = a.off[pB];
+  const int64_t a0 = r_lo & ~(int64_t)3;   // 4-row aligned: every array offset is 16-byte aligned
+  const int64_t nchunks = r_hi > r_lo ? (r_hi - a0 + CH - 1) / CH : 0;
+  auto issue = [&](int64_t c, int buf) {   // one thread: TMA copies of chunk c into stage buffer buf
+    const int64_t start = a0 + c * CH;
+    const uint32_t rows = (uint32_t)min((int64_t)CH, a.m - start);
+    char* sb = stage0 + (size_t)buf * SBYTES;
+    const uint32_t b8 = (rows * 8 + 15) & ~15u;
+    uint32_t total = b8 * NK;
+#pragma unroll
+    for (int s = 0; s < NV; s++) total += (rows * rf_vwidth<SIG, NA>(s) + 15) & ~15u;
+    fence_proxy_async();
+    mbar_expect_tx(&s_bar[buf], total);
+    tma_bulk_g2s(sb, a.rows.k0 + start, b8, &s_bar[buf]);
+    if (NK == 2) tma_bulk_g2s(sb + SOFF_K1, a.rows.k1 + start, b8, &s_bar[buf]);
+#pragma unroll
+    for (int s = 0; s < NV; s++)
+      tma_bulk_g2s(sb + soff_v(s), a.rows.v[s] + start * rf_vwidth<SIG, NA>(s), (rows * rf_vwidth<SIG, NA>(s) + 15) & ~15u, &s_bar[buf]);
+  };
+  if (threadIdx.x == 0) {
+    s_nused = 0;
+    for (int b = 0; b < RF_NBUF; b++) mbar_init(&s_bar[b], 1);
+    mbar_fence_init();
+    if (nchunks > 0) issue(0, 0);
+  }
+  __syncthreads();
+  uint32_t phases = 0;   // bit b: parity of stage buffer b's next completion
+  int p = pA;
+  uint32_t nu = 0;       // claimed slots (= groups alive in the table), block-uniform
+  // every logged group -> the compact group arrays (one reservation per flush), every logged slot reset: the table is EMPTY
+  // afterwards.  Only at a partition boundary: a partial flush breaks the linear-probing chains of the groups that stay.
+  auto flush_all = [&]() {
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      const uint32_t n = s_nused;
+      s_nflush = n;
+      s_obase = n ? atomicAdd(a.gcount, (unsigned long long)n) : 0ull;
+      s_nused = 0;
+    }
+    __syncthreads();
+    const uint32_t n = s_nflush;
+    const unsigned long long ob = s_obase;
+    for (uint32_t u = threadIdx.x; u < n; u += RF_NT) {
+      const int sl = t_used[u];
+      const unsigned long long o = ob + u;
+      a.gk0[o] = t_k0[sl];
+      if (NK == 2) a.gk1[o] = t_k1[sl];
+      uint32_t w[NW > 0 ? NW : 1];
+#pragma unroll
+      for (int j = 0; j < NW; j++) { w[j] = t_w[j * C + sl]; t_w[j * C + sl] = 0; }
+      uint64_t* g = a.gacc + o * LIMBS;
+#pragma unroll
+      for (int k = 0; k < NA; k++) {
+        const int wo = rf_word_off<SIG, NA>(k), lo = rf_limb_off<SIG, NA>(k);
+        const uint32_t kind = rf_kind(SIG, k);
+        const uint64_t l0 = kind == RF_COUNT ? (uint64_t)w[wo] : ((uint64_t)w[wo + 1] << 32 | w[wo]);
+        g[lo] = l0;
+        if (kind == RF_SUMDEC64) g[lo + 1] = (uint64_t)(int64_t)(int32_t)w[wo + 2];
+        if (kind == RF_SUMDEC128) { g[lo + 1] = (uint64_t)w[wo + 3] << 32 | w[wo + 2]; g[lo + 2] = (uint64_t)(int64_t)(int32_t)w[wo + 4]; }
+      }
+      t_state[sl] = 0;
+    }
+    __syncthreads();
+    nu = 0;
+  };
+  for (int64_t c = 0; c < nchunks; c++) {
+    const int buf = (int)(c % RF_NBUF);
+    if (threadIdx.x == 0 && c + 1 < nchunks) issue(c + 1, (int)((c + 1) % RF_NBUF));
+    mbar_wait(&s_bar[buf], (phases >> buf) & 1u);
+    phases ^= 1u << buf;
+    const char* sb = stage0 + (size_t)buf * SBYTES;
+    const int64_t cs = a0 + c * CH;
+    const int64_t lo = max(cs, r_lo), hi = min(cs + CH, r_hi);
+    int claimed = -1;   // the slot this thread claimed in the current segment
+    // row cs + threadIdx.x if it lies in [from, to)
+    auto aggregate_row = [&](int64_t from, int64_t to) {
+      claimed = -1;
+      const int64_t r = cs + threadIdx.x;
+      if (r < from || r >= to) return;
+      const int li = threadIdx.x;
+      const uint64_t k0 = reinterpret_cast<const uint64_t*>(sb)[li];
+      const uint64_t k1 = NK == 2 ? reinterpret_cast<const uint64_t*>(sb + SOFF_K1)[li] : 0ull;
+      uint32_t idx = (uint32_t)rg_hash(k0, k1) & (uint32_t)(C - 1);
+      int probes = 0;
+      // A slot claimed in this chunk or the previous one (no RG_READY yet) is compared through that chunk's stage buffer, which
+      // stays intact for two chunks (three buffers, one prefetched); its table key is only read once RG_READY is set, after the
+      // barrier that ends the claiming chunk.  No memory fence and no volatile key read per row.
+      while (true) {
+        uint32_t st = *reinterpret_cast<volatile uint32_t*>(&t_state[idx]);
+        if (st == 0) {
+          const uint32_t old = atomicCAS(&t_state[idx], 0u, (uint32_t)(buf * CH + li + 1));
+          if (old == 0) {
+            t_k0[idx] = k0;
+            if (NK == 2) t_k1[idx] = k1;
+            t_used[atomicAdd(&s_nused, 1u)] = (uint16_t)idx;
+            claimed = (int)idx;
+            break;
+          }
+          st = old;
+        }
+        bool same;
+        if (st & RG_READY) same = t_k0[idx] == k0 && (NK == 1 || t_k1[idx] == k1);
+        else {
+          const int q = (int)st - 1, qb = q / CH, qi = q % CH;
+          const char* ob = stage0 + (size_t)qb * SBYTES;
+          same = reinterpret_cast<const uint64_t*>(ob)[qi] == k0 && (NK == 1 || reinterpret_cast<const uint64_t*>(ob + SOFF_K1)[qi] == k1);
+        }
+        if (same) break;
+        idx = (idx + 1) & (uint32_t)(C - 1);
+        if (++probes > C / 2) { atomicExch(a.overflow, 1); return; }
+      }
+#pragma unroll
+      for (int k = 0; k < NA; k++) {
+        const uint32_t kind = rf_kind(SIG, k);
+        uint32_t* w = t_w + (size_t)rf_word_off<SIG, NA>(k) * C;
+        if (kind == RF_COUNT) { atomicAdd(&w[idx], 1u); continue; }
+        const char* vp = sb + soff_v(rf_slot(SIG, k));
+        if (kind == RF_SUMDEC128) {
+          const uint4 v = reinterpret_cast<const uint4*>(vp)[li];
+          const uint32_t x[4] = {v.x, v.y, v.z, v.w};
+          rf_add<4>(w, C, (int)idx, x, true);
+        } else {
+          const uint2 v = reinterpret_cast<const uint2*>(vp)[li];
+          const uint32_t x[2] = {v.x, v.y};
+          rf_add<2>(w, C, (int)idx, x, kind == RF_SUMDEC64);
+        }
+      }
+    };
+    int64_t from = lo;
+    if (nu >= (uint32_t)(C / 4)) {
+      while (p < pB && (int64_t)a.off[p + 1] <= lo) p++;   // a.off[p] <= lo < a.off[p + 1]
+      if (p < pB) {
+        const int64_t bnd = (int64_t)a.off[p] == lo ? lo : (int64_t)a.off[p + 1];   // the first partition boundary at or after lo
+        if (bnd <= hi) {
+          aggregate_row(lo, bnd);
+          flush_all();
+          from = bnd;
+        }
+      }
+    }
+    aggregate_row(from, hi);
+    if (c + 1 == nchunks) { flush_all(); claimed = -1; }
+    // the chunk is aggregated: its keys are in the table.  The count is block-uniform, and nobody can claim a slot of the next
+    // chunk before every thread has passed this barrier.
+    nu += (uint32_t)__syncthreads_count(claimed >= 0);
+    if (claimed >= 0) t_state[claimed] = RG_READY;   // from now on compared through the table
+  }
+}
+
 struct RGKeyOut { void* data[MAX_KEYS]; int32_t width[MAX_KEYS]; };
 __global__ void radix_finalize_kernel(const __grid_constant__ AggPlan plan, const __grid_constant__ RGPlan rp, int64_t ngroups, const uint64_t* __restrict__ gk0,
                                       const uint64_t* __restrict__ gk1, const uint64_t* __restrict__ gacc, const uint32_t* __restrict__ gnvalid,
@@ -1053,6 +1281,46 @@ static void make_agg_outputs(const AggPlan& plan, const Program* prog, const b2_
   }
 }
 
+// the instantiations of radix_agg_fixed_kernel: q3's DECIMAL128 sum, the other sums and counts, distinct; one or two key words
+struct RFKernel {
+  int nk, nv, na;
+  uint32_t sig;
+  void (*fn)(const RGAgg);
+  int stage_bytes, slot_bytes;
+};
+template <int NK, int NV, int NA, uint32_t SIG>
+static RFKernel rf_kernel() {
+  return {NK, NV, NA, SIG, radix_agg_fixed_kernel<NK, NV, NA, SIG>, rf_stage_bytes<NK, NV, NA, SIG>(),
+          8 * NK + 4 * rf_word_off<SIG, NA>(NA) + 4 + 2};   // keys, accumulator words, state, claimed-slot log
+}
+#define RF_SHAPES(NK)                                                                        \
+  rf_kernel<NK, 1, 1, rf_agg(RF_SUMDEC128, 0, 0)>(), rf_kernel<NK, 1, 1, rf_agg(RF_SUMDEC64, 0, 0)>(), \
+  rf_kernel<NK, 1, 1, rf_agg(RF_SUM64, 0, 0)>(), rf_kernel<NK, 1, 2, rf_agg(RF_SUM64, 0, 0) | rf_agg(RF_COUNT, 0, 1)>(), \
+  rf_kernel<NK, 0, 1, rf_agg(RF_COUNT, 0, 0)>(), rf_kernel<NK, 0, 0, 0u>()
+
+// the specialised kernel for this plan, or nullptr: MIN / MAX, nullable values, counts of a column no sum reads, other mixes
+static const RFKernel* rf_select(const AggPlan& plan, const RGPlan& rp) {
+  static const RFKernel table[] = {RF_SHAPES(1), RF_SHAPES(2)};
+  if (rp.use_vbits || plan.naggs > 4) return nullptr;
+  uint32_t sig = 0;
+  int vwidth[RG_MAX_VALS] = {0};
+  for (int k = 0; k < plan.naggs; k++) {
+    const AggD& a = plan.aggs[k];
+    if (a.track_valid || a.is_float) return nullptr;
+    uint32_t kind;
+    if (a.kind == B2_AGG_COUNT || a.kind == B2_AGG_COUNT_ALL) kind = RF_COUNT;
+    else if (a.kind == B2_AGG_SUM) kind = a.nlimbs == 1 ? RF_SUM64 : a.nlimbs == 2 ? RF_SUMDEC64 : RF_SUMDEC128;
+    else return nullptr;
+    const int slot = kind == RF_COUNT ? 0 : rp.agg_val[k];
+    if (kind != RF_COUNT) vwidth[slot] = kind == RF_SUMDEC128 ? 16 : 8;
+    sig |= rf_agg(kind, (uint32_t)slot, k);
+  }
+  for (int s = 0; s < rp.nvals; s++) if (vwidth[s] != rp.val[s].width) return nullptr;
+  for (const RFKernel& f : table)
+    if (f.nk == 1 + rp.has_k1 && f.nv == rp.nvals && f.na == plan.naggs && f.sig == sig) return &f;
+  return nullptr;
+}
+
 // the radix-partitioned regime; nullptr = not applicable (or a partition overflowed its table): the caller falls back
 static Table* radix_groupby(const Program* prog, const Table* t, const AggPlan& plan, const b2_agg_spec* specs, const std::vector<int>& key_table_cols,
                             const VMInputs& in) {
@@ -1093,8 +1361,22 @@ static Table* radix_groupby(const Program* prog, const Table* t, const AggPlan& 
   sbytes = (sbytes + 127) & ~127;
   int C = 2048;
   while (C >= 1024 && C * slot_bytes + 2 * sbytes + 512 > 200 * 1024) C >>= 1;
+  int agg_smem = C * slot_bytes + 2 * sbytes + 512;
+  // the specialised kernel takes the largest table the device's shared memory holds next to its three stage buffers
+  const RFKernel* rf = rf_select(plan, rp);
+  if (rf) {
+    int dev = 0, optin = 0;
+    CUDA_CHECK(cudaGetDevice(&dev));
+    CUDA_CHECK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+    cudaFuncAttributes fa;
+    CUDA_CHECK(cudaFuncGetAttributes(&fa, rf->fn));
+    const int budget = optin - (int)fa.sharedSizeBytes;
+    int rc = 8192;
+    while (rc >= 1024 && rc * rf->slot_bytes + 128 + RF_NBUF * rf->stage_bytes > budget) rc >>= 1;
+    if (rc >= 1024) { C = rc; agg_smem = rc * rf->slot_bytes + 128 + RF_NBUF * rf->stage_bytes; }
+    else rf = nullptr;
+  }
   if (C < 1024) return nullptr;
-  const int agg_smem = C * slot_bytes + 2 * sbytes + 512;
 
   // 1. materialise the (filtered, projected) rows
   struct Side { DevBuf h, k0, k1, v[RG_MAX_VALS], vbits; };
@@ -1133,19 +1415,17 @@ static Table* radix_groupby(const Program* prog, const Table* t, const AggPlan& 
   Side* cur = &A; Side* oth = &B;
   if (P > 1) {
     alloc_side(B);
-    DevBuf pid((size_t)m * 4);
-    // LSD passes of at most 8 bits each (the <= 256-way scatter is the fast one), stable, so the final order is by h & (P - 1)
+    // LSD passes of at most 8 bits each (the <= 256-way scatter is the fast one), stable, so the final order is by h & (P - 1);
+    // each pass takes its digit straight from the hash array it moves
     for (int shift = 0; shift < lgP;) {
       const int bits = std::min(8, lgP - shift);
-      rg_digit_kernel<<<grid_for(m, 256), 256, 0, stream()>>>(cur->h.as<uint32_t>(), m, shift, (1u << bits) - 1u, pid.as<int32_t>());
-      count_launch();
       ScatterCols sc; memset(&sc, 0, sizeof(sc));
       auto add = [&](DevBuf& i, DevBuf& o, int w) { sc.width[sc.n] = w; sc.in[sc.n] = i.p; sc.out[sc.n] = o.p; sc.n++; };
       add(cur->h, oth->h, 4); add(cur->k0, oth->k0, 8);
       if (rp.has_k1) add(cur->k1, oth->k1, 8);
       for (int s2 = 0; s2 < rp.nvals; s2++) add(cur->v[s2], oth->v[s2], rp.val[s2].width);
       if (rp.use_vbits) add(cur->vbits, oth->vbits, 4);
-      partition_scatter_arrays(pid.as<int32_t>(), m, 1 << bits, sc);
+      partition_scatter_by_hash(cur->h.as<uint32_t>(), shift, bits, m, sc);
       std::swap(cur, oth);
       shift += bits;
     }
@@ -1160,7 +1440,13 @@ static Table* radix_groupby(const Program* prog, const Table* t, const AggPlan& 
   ap.rows = rows_of(*cur); ap.off = off.as<int32_t>(); ap.P = (int32_t)P; ap.C = C; ap.m = m;
   ap.gk0 = gk0.as<uint64_t>(); ap.gk1 = gk1.as<uint64_t>(); ap.gacc = gacc.as<uint64_t>(); ap.gnvalid = gnv.as<uint32_t>();
   ap.gcount = counter.as<unsigned long long>() + 1; ap.overflow = ovf.as<int32_t>();
-  {
+  if (rf) {
+    CUDA_CHECK(cudaFuncSetAttribute(rf->fn, cudaFuncAttributeMaxDynamicSharedMemorySize, agg_smem));
+    KernelTimer kt("radix_agg_fixed_kernel");
+    rf->fn<<<(int)std::min<int64_t>(P, sm_count()), RF_NT, agg_smem, stream()>>>(ap);
+    CUDA_CHECK(cudaGetLastError());
+    count_launch();
+  } else {
     CUDA_CHECK(cudaFuncSetAttribute(radix_agg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, agg_smem));
     KernelTimer kt("radix_agg_kernel");
     radix_agg_kernel<<<(int)std::min<int64_t>(P, sm_count()), RG_NT, agg_smem, stream()>>>(plan, rp, ap);

@@ -51,7 +51,22 @@ Table* gather_table(const Table* t, const int32_t* d_map, int64_t n, bool nullif
 // place.  Reads are coalesced, writes are coalesced per run of equal ids.  Other columns (strings, nullable) go
 // through the gather map the same kernel can emit.  Replaces id->key expansion + radix pass + random-read gather.
 constexpr int PT_NT = 256, PT_STEPS = 16, PT_TILE = PT_NT * PT_STEPS, PT_MAXP = 1024;   // PT_MAXC, ScatterCols: prim.cuh
-__global__ void __launch_bounds__(PT_NT) part_tile_hist_kernel(const int32_t* __restrict__ pids, int64_t n, int32_t nparts, int64_t ntiles,
+// Where a row's partition id comes from: an id array (Table.partition), or a digit of a 32-bit hash array (the radix group-by's
+// passes, which move that hash array anyway: no separate digit pass and no id array)
+struct PidArray {
+  const int32_t* p;
+  __device__ __forceinline__ int32_t operator()(int64_t i) const { return p[i]; }
+};
+struct HashDigit {
+  const uint32_t* h;
+  int shift;
+  uint32_t mask;
+  // default cache policy: the scatter moves the hash array itself right after, and that read should hit L2
+  __device__ __forceinline__ int32_t operator()(int64_t i) const { return (int32_t)((h[i] >> shift) & mask); }
+};
+
+template <typename Pid>
+__global__ void __launch_bounds__(PT_NT) part_tile_hist_kernel(const Pid pids, int64_t n, int32_t nparts, int64_t ntiles,
                                                                int32_t* __restrict__ tile_cnt) {
   __shared__ int32_t h[PT_MAXP];
   for (int p = threadIdx.x; p < nparts; p += PT_NT) h[p] = 0;
@@ -59,7 +74,7 @@ __global__ void __launch_bounds__(PT_NT) part_tile_hist_kernel(const int32_t* __
   const int64_t tile = blockIdx.x;
   for (int j = 0; j < PT_STEPS; j++) {
     const int64_t i = tile * PT_TILE + (int64_t)j * PT_NT + threadIdx.x;
-    if (i < n) { const int32_t p = pids[i]; if ((uint32_t)p < (uint32_t)nparts) atomicAdd(&h[p], 1); }
+    if (i < n) { const int32_t p = pids(i); if ((uint32_t)p < (uint32_t)nparts) atomicAdd(&h[p], 1); }
   }
   __syncthreads();
   for (int p = threadIdx.x; p < nparts; p += PT_NT) tile_cnt[(int64_t)p * ntiles + tile] = h[p];
@@ -165,7 +180,7 @@ __device__ __forceinline__ void ps_move(const T* __restrict__ in, T* __restrict_
   }
   __syncthreads();
 }
-__global__ void __launch_bounds__(PT_NT, 4) part_scatter2_kernel(const int32_t* __restrict__ pids, int64_t n, int32_t nparts, int64_t ntiles,
+__global__ void __launch_bounds__(PT_NT, 4) part_scatter2_kernel(const HashDigit pids, int64_t n, int32_t nparts, int64_t ntiles,
                                                               const int32_t* __restrict__ base, const __grid_constant__ ScatterCols sc) {
   extern __shared__ __align__(16) char ps_stage[];    // PT_TILE x widest array
   __shared__ uint32_t s_wh[PS_WARPS][256];
@@ -183,7 +198,7 @@ __global__ void __launch_bounds__(PT_NT, 4) part_scatter2_kernel(const int32_t* 
   for (int r = 0; r < PT_STEPS; r++) {
     const int64_t i = wbase + r * 32 + lane;
     const bool in = i < n;
-    const uint32_t d = in ? (uint32_t)__ldcs(&pids[i]) : 256u + lane;   // out-of-range lanes match nobody
+    const uint32_t d = in ? (uint32_t)pids(i) : 256u + lane;   // out-of-range lanes match nobody
     const uint32_t m = __match_any_sync(0xffffffffu, d);
     const uint32_t before = __popc(m & ((1u << lane) - 1u));
     uint32_t prev = 0;
@@ -244,7 +259,7 @@ static Table* partition_table_direct(const Table* t, const int32_t* d_pids, int3
   DevBuf cnt((size_t)(cells + 1) * 4);
   {
     KernelTimer kt("part_tile_hist_kernel");
-    part_tile_hist_kernel<<<(int)ntiles, PT_NT, 0, stream()>>>(d_pids, n, nparts, ntiles, cnt.as<int32_t>());
+    part_tile_hist_kernel<<<(int)ntiles, PT_NT, 0, stream()>>>(PidArray{d_pids}, n, nparts, ntiles, cnt.as<int32_t>());
     CUDA_CHECK(cudaGetLastError());
     count_launch();
   }
@@ -284,32 +299,30 @@ static Table* partition_table_direct(const Table* t, const int32_t* d_pids, int3
   return new_table(outs.release());
 }
 
-// raw-array form (radix group-by, agg.cu): stable scatter of up to PT_MAXC fixed-width arrays by partition id (< 1024)
-void partition_scatter_arrays(const int32_t* d_pids, int64_t n, int32_t nparts, const ScatterCols& sc) {
+// raw-array form (radix group-by, agg.cu): stable scatter of up to PT_MAXC fixed-width arrays by the digit
+// (d_hash[i] >> shift) & (2^bits - 1), bits <= 8
+void partition_scatter_by_hash(const uint32_t* d_hash, int shift, int bits, int64_t n, const ScatterCols& sc) {
   if (n == 0) return;
-  B2_CHECK(nparts >= 1 && nparts <= PT_MAXP, "partition_scatter_arrays: 1..1024 partitions");
+  B2_CHECK(bits >= 1 && bits <= 8, "partition_scatter_by_hash: 1..8 digit bits");
+  const int32_t nparts = 1 << bits;
+  const HashDigit pid{d_hash, shift, (uint32_t)nparts - 1u};
   const int64_t ntiles = (n + PT_TILE - 1) / PT_TILE;
   const int64_t cells = (int64_t)nparts * ntiles;
   DevBuf cnt((size_t)(cells + 1) * 4);
   {
     KernelTimer kt("part_tile_hist_kernel");
-    part_tile_hist_kernel<<<(int)ntiles, PT_NT, 0, stream()>>>(d_pids, n, nparts, ntiles, cnt.as<int32_t>());
+    part_tile_hist_kernel<<<(int)ntiles, PT_NT, 0, stream()>>>(pid, n, nparts, ntiles, cnt.as<int32_t>());
     CUDA_CHECK(cudaGetLastError());
     count_launch();
   }
   DevBuf sums = exclusive_scan<int32_t, int32_t>(cnt.as<int32_t>(), cnt.as<int32_t>(), cells, true);
-  if (nparts <= 256) {
+  {
     int maxw = 1;
     for (int c = 0; c < sc.n; c++) maxw = std::max(maxw, sc.width[c]);
     const int smem = PT_TILE * maxw;
     if (smem > 32 * 1024) CUDA_CHECK(cudaFuncSetAttribute(part_scatter2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     KernelTimer kt("part_scatter2_kernel");
-    part_scatter2_kernel<<<(int)ntiles, PT_NT, smem, stream()>>>(d_pids, n, nparts, ntiles, cnt.as<int32_t>(), sc);
-    CUDA_CHECK(cudaGetLastError());
-    count_launch();
-  } else {
-    KernelTimer kt("part_scatter_kernel");
-    part_scatter_kernel<<<(int)ntiles, PT_NT, 0, stream()>>>(d_pids, n, nparts, ntiles, cnt.as<int32_t>(), sc, nullptr);
+    part_scatter2_kernel<<<(int)ntiles, PT_NT, smem, stream()>>>(pid, n, nparts, ntiles, cnt.as<int32_t>(), sc);
     CUDA_CHECK(cudaGetLastError());
     count_launch();
   }

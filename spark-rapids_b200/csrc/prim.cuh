@@ -14,7 +14,8 @@ struct ScatterCols {
   const void* in[PT_MAXC];
   void* out[PT_MAXC];
 };
-void partition_scatter_arrays(const int32_t* d_pids, int64_t n, int32_t nparts, const ScatterCols& sc);
+// the partition of row i is the digit (d_hash[i] >> shift) & (2^bits - 1), bits <= 8
+void partition_scatter_by_hash(const uint32_t* d_hash, int shift, int bits, int64_t n, const ScatterCols& sc);
 
 #ifdef __CUDACC__
 constexpr int SCAN_NT = 256;
