@@ -401,9 +401,12 @@ int b2_exec_project(b2_handle child, b2_handle program, b2_handle* out);        
 /* GpuExpandExec (GpuExpandExec.scala): each batch projected once per projection list, results stacked (GROUPING SETS,
  * several COUNT(DISTINCT)); all projection programs must produce the same output types */
 int b2_exec_expand(b2_handle child, const b2_handle* projection_programs, int32_t nprojections, b2_handle* out);
-/* GpuHashAggregateExec (GpuAggregateExec.scala:1942-2085).  merge_mode 0: update aggregates over the
- * program's outputs (Partial/Complete); 1: input batches are aggregation buffers, keys leading (Final) */
-int b2_exec_hash_aggregate(b2_handle child, b2_handle program, int32_t has_predicate, int32_t merge_mode,
+/* GpuHashAggregateExec (GpuAggregateExec.scala:1942-2085).  PARTIAL and COMPLETE update the aggregates over
+ * the program's outputs; FINAL merges aggregation buffers.  A buffer (PARTIAL's output, FINAL's input) is the
+ * keys, one column per aggregate, then one INT64 count of valid inputs per decimal SUM, in aggregate order
+ * (Spark's isEmpty): a NULL partial sum with a nonzero count overflowed, and makes the merged sum NULL. */
+typedef enum { B2_AGG_MODE_PARTIAL = 0, B2_AGG_MODE_FINAL = 1, B2_AGG_MODE_COMPLETE = 2 } b2_agg_mode;
+int b2_exec_hash_aggregate(b2_handle child, b2_handle program, int32_t has_predicate, int32_t mode,
                            const int32_t* keys, int32_t nkeys, const b2_agg_spec* aggs, int32_t naggs, b2_handle* out);
 /* GpuShuffledHashJoinExec (GpuShuffledHashJoinExec.scala:228-385): output = stream columns ++ build columns */
 int b2_exec_shuffled_hash_join(b2_handle stream_child, b2_handle build_child, const int32_t* stream_keys,

@@ -16,6 +16,7 @@
 //   GpuSortExec / GpuTopN     GpuSortExec.scala:87-165 (each-batch | full), limit.scala:234-330
 //   GpuCoalesceBatches        GpuCoalesceBatches.scala:160-239 (TargetSize goal by rows)
 //   GpuShuffleExchangeExec    GpuShuffleExchangeExecBase.scala:384-536 with the NCCL all-to-all
+#include <algorithm>
 #include <chrono>
 #include <deque>
 #include "vm.cuh"
@@ -263,14 +264,54 @@ struct GpuExpandExec : GpuExec {
   }
 };
 
+// A partial decimal sum that overflowed is NULL although its group saw valid input (Spark's buffer (sum, isEmpty) with sum NULL
+// and isEmpty false); a merge must then give NULL, whereas a NULL partial of an empty / all-NULL group is skipped.  Marks the
+// first kind of row: flag[r] = sum[r] is NULL and (no count column, or count[r] > 0); *npoisoned counts them.
+__global__ void poisoned_sums_kernel(const uint32_t* __restrict__ sum_valid, const int64_t* __restrict__ count, int64_t n, int8_t* __restrict__ flag,
+                                     unsigned long long* __restrict__ npoisoned) {
+  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < n; r += (int64_t)gridDim.x * blockDim.x) {
+    const bool p = !((sum_valid[r >> 5] >> (r & 31)) & 1u) && (count == nullptr || count[r] > 0);
+    flag[r] = p;
+    if (p) atomicAdd(npoisoned, 1ull);
+  }
+}
+// clears the validity bit of every row whose merged flag (MAX of the partials' flags) is set
+__global__ void clear_poisoned_kernel(uint32_t* __restrict__ valid, const int8_t* __restrict__ flag, int64_t n) {
+  for (int64_t w = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; w < (n + 31) >> 5; w += (int64_t)gridDim.x * blockDim.x) {
+    uint32_t m = 0;
+    for (int b = 0; b < 32 && w * 32 + b < n; b++) m |= (uint32_t)(flag[w * 32 + b] != 0) << b;
+    valid[w] &= ~m;
+  }
+}
+
 // aggregate modes as in Spark: Partial/Complete run the update aggregates on raw input, Final merges
-// partial buffers (SUM of sums, SUM of counts, MIN of mins, MAX of maxes)
+// partial buffers (SUM of sums, SUM of counts, MIN of mins, MAX of maxes).  A partial buffer is the keys, one column per
+// aggregate, then one INT64 count of valid inputs per decimal SUM (Spark's isEmpty, GpuDecimalSum).  Complete mode keeps
+// that count between its own passes only, and only where a NULL partial sum may also mean an empty group.
 struct GpuHashAggregateExec : GpuExec {
   Program* program = nullptr;  // pre-step projection (+ fused predicate as output 0) for update mode; null in merge mode
-  bool has_pred = false, merge_mode = false, done = false;
+  int mode = B2_AGG_MODE_PARTIAL;
+  bool has_pred = false, done = false;
   std::vector<int> keys;               // update: program outputs; merge: leading input columns
   std::vector<b2_agg_spec> aggs;       // update: columns = program outputs; merge: columns = input columns
+  std::vector<int> counted;            // the decimal SUMs whose partials carry a count column, in column order
 
+  static bool decimal_sum(const b2_agg_spec& s) { return s.kind == B2_AGG_SUM && (s.out_dtype == B2_DECIMAL64 || s.out_dtype == B2_DECIMAL128); }
+  void init_counted() {
+    for (int i = 0; i < (int)aggs.size(); i++) {
+      if (!decimal_sum(aggs[i])) continue;
+      // complete mode, keyed, NOT NULL input: every group of a partial saw a valid value, so a NULL sum is an overflow
+      const int o = aggs[i].column + (has_pred ? 1 : 0);
+      if (mode == B2_AGG_MODE_COMPLETE) B2_CHECK(o >= 0 && o < (int)program->out_nullable.size(), "aggregate input index out of range");
+      const bool need = mode != B2_AGG_MODE_COMPLETE || keys.empty() || program->out_nullable[o];
+      if (need) counted.push_back(i);
+    }
+  }
+  std::vector<b2_agg_spec> update_specs() const {
+    std::vector<b2_agg_spec> u = aggs;
+    for (int i : counted) u.push_back(b2_agg_spec{B2_AGG_COUNT, aggs[i].column, B2_INT64, 0, 0});
+    return u;
+  }
   static std::vector<b2_agg_spec> merge_specs(const std::vector<b2_agg_spec>& a, int nkeys) {
     std::vector<b2_agg_spec> m = a;
     for (size_t i = 0; i < m.size(); i++) {
@@ -279,19 +320,66 @@ struct GpuHashAggregateExec : GpuExec {
     }
     return m;
   }
-  Table* merge(const Table* t) {  // keys are the leading columns
-    std::vector<int> cols, key_outs;
-    for (int k = 0; k < (int)keys.size(); k++) { key_outs.push_back(k); cols.push_back(k); }
-    std::vector<b2_agg_spec> m = merge_specs(aggs, (int)keys.size());
-    for (auto& s : m) cols.push_back(s.column);
-    std::unique_ptr<Program> p(make_passthrough_program(t, cols));
-    return scan_aggregate(p.get(), false, t, key_outs.data(), (int)key_outs.size(), m.data(), (int)m.size());
+  // a complete-mode result of one partial: the keys and the aggregates, without the counts (takes t)
+  Table* without_counts(Table* t) {
+    if (mode == B2_AGG_MODE_PARTIAL || counted.empty()) return t;
+    TableRef in(t);
+    std::vector<Column*> cols(t->cols.begin(), t->cols.begin() + keys.size() + aggs.size());
+    for (Column* c : cols) col_incref(c);
+    return new_table(std::move(cols));
+  }
+  Table* merge(const Table* t) {  // keys are the leading columns, then the aggregates, then the counts
+    const int nk = (int)keys.size(), na = (int)aggs.size(), nc = (int)counted.size();
+    std::vector<b2_agg_spec> m = merge_specs(update_specs(), nk);
+    // flag the partial decimal sums that overflowed; only when there are any does the merge carry them (MAX of the flags)
+    ColsGuard flags;
+    std::vector<int> flagged;
+    DevBuf npois(8);
+    CUDA_CHECK(cudaMemsetAsync(npois.p, 0, 8, stream()));
+    for (int i = 0; i < na; i++) {
+      const Column* s = t->cols[nk + i];
+      if (!decimal_sum(aggs[i]) || !s->nullable() || t->rows == 0) continue;
+      const int j = (int)(std::find(counted.begin(), counted.end(), i) - counted.begin());
+      const int64_t* count = j < nc ? t->cols[nk + na + j]->data.as<int64_t>() : nullptr;
+      Column* f = new_column(B2_INT8, 0, t->rows, false);
+      flags.v.push_back(f); flagged.push_back(i);
+      poisoned_sums_kernel<<<grid_for(t->rows, 256), 256, 0, stream()>>>(s->validity(), count, t->rows, f->data.as<int8_t>(), npois.as<unsigned long long>());
+      CUDA_CHECK(cudaGetLastError());
+      count_launch();
+    }
+    unsigned long long hpois = 0;
+    if (!flagged.empty()) { d2h(&hpois, npois.p, 1); sync(); }
+    if (hpois == 0) flagged.clear();
+    std::vector<Column*> in_cols(t->cols.begin(), t->cols.end());
+    for (size_t q = 0; q < flagged.size(); q++) {
+      in_cols.push_back(flags.v[q]);
+      m.push_back(b2_agg_spec{B2_AGG_MAX, (int)in_cols.size() - 1, B2_INT8, 0, 0});
+    }
+    for (Column* c : in_cols) col_incref(c);
+    TableRef src(new_table(std::move(in_cols)));
+    std::vector<int> cols, key_outs;   // every input column once, in order: program output i is column i
+    for (int k = 0; k < nk; k++) key_outs.push_back(k);
+    for (int c = 0; c < nk + (int)m.size(); c++) cols.push_back(c);
+    std::unique_ptr<Program> p(make_passthrough_program(src.t, cols));
+    TableRef r(scan_aggregate(p.get(), false, src.t, key_outs.data(), nk, m.data(), (int)m.size()));
+    for (size_t q = 0; q < flagged.size(); q++) {
+      Column* s = r.t->cols[nk + flagged[q]];
+      clear_poisoned_kernel<<<grid_for((r.t->rows + 31) / 32, 256), 256, 0, stream()>>>(s->valid.as<uint32_t>(), r.t->cols[nk + na + nc + q]->data.as<int8_t>(),
+                                                                                        r.t->rows);
+      CUDA_CHECK(cudaGetLastError());
+      count_launch();
+      s->null_count = -1;
+    }
+    std::vector<Column*> out(r.t->cols.begin(), r.t->cols.begin() + nk + na + (mode == B2_AGG_MODE_PARTIAL ? nc : 0));
+    for (Column* c : out) col_incref(c);
+    return new_table(std::move(out));
   }
   // first-pass aggregation of one input batch; when the device cannot hold it the batch is split in halves, each half
   // yields its own partial (the merge pass combines them like any other pair of partials)
   void first_pass(const Table* in, std::vector<TableRef>& partials, int depth) {
     try {
-      partials.emplace_back(with_retry([&] { return scan_aggregate(program, has_pred, in, keys.data(), (int)keys.size(), aggs.data(), (int)aggs.size()); }));
+      const std::vector<b2_agg_spec> u = update_specs();
+      partials.emplace_back(with_retry([&] { return scan_aggregate(program, has_pred, in, keys.data(), (int)keys.size(), u.data(), (int)u.size()); }));
     } catch (const Error& e) {
       if (!splittable(e) || in->rows < 2 || depth >= 12) throw;
       note_split();
@@ -307,15 +395,15 @@ struct GpuHashAggregateExec : GpuExec {
     while (true) {
       TableRef in(children[0]->next());
       if (!in.t) break;
-      if (merge_mode) partials.emplace_back(in.release());   // inputs already are aggregation buffers
+      if (mode == B2_AGG_MODE_FINAL) partials.emplace_back(in.release());   // inputs already are aggregation buffers
       else first_pass(in.t, partials, 0);
     }
     if (partials.empty()) {
       // a keyless aggregate over no batches still emits its initial-value row (GpuAggregateExec.scala:1107-1126)
-      if (!keys.empty() || merge_mode) return nullptr;
+      if (!keys.empty() || mode == B2_AGG_MODE_FINAL) return nullptr;
       throw Error(B2_ERR_UNSUPPORTED, "keyless aggregate over zero input batches needs the input schema");
     }
-    if (partials.size() == 1 && !merge_mode) return partials[0].release();
+    if (partials.size() == 1 && mode != B2_AGG_MODE_FINAL) return without_counts(partials[0].release());
     std::vector<const Table*> ts;
     for (auto& p : partials) ts.push_back(p.t);
     TableRef cat(concat_tables(ts));
@@ -836,15 +924,17 @@ int b2_exec_project(b2_handle child, b2_handle program, b2_handle* out) {
   *out = to_handle(e);
   B2_CATCH
 }
-int b2_exec_hash_aggregate(b2_handle child, b2_handle program, int32_t has_predicate, int32_t merge_mode, const int32_t* keys, int32_t nkeys,
+int b2_exec_hash_aggregate(b2_handle child, b2_handle program, int32_t has_predicate, int32_t mode, const int32_t* keys, int32_t nkeys,
                            const b2_agg_spec* aggs, int32_t naggs, b2_handle* out) {
   B2_TRY
-  auto* e = new GpuHashAggregateExec();
-  e->add_child(exec_from(child));
-  e->program = merge_mode ? nullptr : program_from(program);
-  e->has_pred = has_predicate != 0; e->merge_mode = merge_mode != 0;
+  B2_CHECK(mode == B2_AGG_MODE_PARTIAL || mode == B2_AGG_MODE_FINAL || mode == B2_AGG_MODE_COMPLETE, "unknown aggregate mode");
+  std::unique_ptr<GpuHashAggregateExec> e(new GpuHashAggregateExec());
+  e->program = mode == B2_AGG_MODE_FINAL ? nullptr : program_from(program);
+  e->has_pred = has_predicate != 0; e->mode = mode;
   e->keys.assign(keys, keys + nkeys); e->aggs.assign(aggs, aggs + naggs);
-  *out = to_handle(e);
+  e->init_counted();
+  e->add_child(exec_from(child));
+  *out = to_handle(e.release());
   B2_CATCH
 }
 int b2_exec_shuffled_hash_join(b2_handle stream_child, b2_handle build_child, const int32_t* stream_keys, const int32_t* build_keys, int32_t nkeys,

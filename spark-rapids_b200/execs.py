@@ -125,15 +125,18 @@ def GpuExpandExec(projections, child):
 
 def GpuHashAggregateExec(child, grouping, aggregates, pre_project=None, condition=None, mode="partial"):
     """mode 'partial'/'complete': update aggregates over `pre_project` expressions (with `condition`
-    fused in as the child filter); 'final': merge aggregation buffers whose keys lead the input."""
+    fused in as the child filter); 'final': merge aggregation buffers whose keys lead the input.
+    A 'partial' output (a 'final' input) is the keys, one column per aggregate, then one INT64 count of
+    valid inputs per decimal SUM (Spark's isEmpty), so that a partial sum that overflowed stays NULL."""
+    code = {"partial": 0, "final": 1, "complete": 2}[mode]
     if mode == "final":
-        return _new(lib.b2_exec_hash_aggregate, child.h, ctypes.c_int64(0), 0, 1, m._i32s(grouping), len(grouping), m._agg_specs(aggregates),
+        return _new(lib.b2_exec_hash_aggregate, child.h, ctypes.c_int64(0), 0, code, m._i32s(grouping), len(grouping), m._agg_specs(aggregates),
                     len(aggregates), keep=[child])
     if isinstance(pre_project, m.Program):    # compiled once per plan (output 0 is the fused condition when `condition` is truthy)
         prog = pre_project
     else:
         prog = m.Program(([condition] if condition is not None else []) + list(pre_project))
-    return _new(lib.b2_exec_hash_aggregate, child.h, prog.h, int(condition is not None), 0, m._i32s(grouping), len(grouping),
+    return _new(lib.b2_exec_hash_aggregate, child.h, prog.h, int(condition is not None), code, m._i32s(grouping), len(grouping),
                 m._agg_specs(aggregates), len(aggregates), keep=[prog, child])
 
 

@@ -290,3 +290,62 @@ def test_expand_exec_two_count_distincts(b2):
     da = len({x for x in a.to_pylist() if x is not None}); db = len({y for y in b.to_pylist() if y is not None})
     distinct = {r for r in rows}
     assert sum(1 for r in distinct if r[2] == 1 and r[0] is not None) == da and sum(1 for r in distinct if r[2] == 2 and r[1] is not None) == db
+
+
+def _dec_batches(b2, rows_per_batch, nullable):
+    """batches of (INT64 key, DECIMAL128(38,0) value) rows; a value of None is NULL"""
+    out = []
+    for rows in rows_per_batch:
+        k = np.array([r[0] for r in rows], dtype=np.int64)
+        v = np.array([0 if r[1] is None else r[1] for r in rows], dtype=object)
+        ok = np.array([r[1] is not None for r in rows])
+        out.append(b2.Table.from_columns([b2.Column.from_numpy(k), b2.Column.from_numpy(v, dtype=b2.DECIMAL128, valid=ok if nullable else None)]))
+    return out
+
+
+@pytest.mark.parametrize("nullable", [False, True])
+@pytest.mark.parametrize("keyed", [True, False])
+@pytest.mark.parametrize("plan", ["complete", "partial_exchange_final"])
+def test_decimal_sum_overflow_in_one_batch_stays_null(b2, plan, keyed, nullable):
+    """SUM(d), d DECIMAL(38,0), result precision 38, over two batches.  Key 1: batch 1 holds 6e37 + 6e37 (its partial
+    overflows, NULL), batch 2 holds 1: Spark's result is NULL (buffer (sum, isEmpty): sum NULL and isEmpty false), and so
+    is the exact total.  A merge that skipped the NULL partial would return 1.  Key 2 sums normally; key 3 (nullable
+    input) has only a NULL in batch 1, an empty partial that the merge must skip.
+    Not pinned: a batch that overflows while the exact total fits (6e37 + 6e37 - 6e37).  This gives NULL, but Spark
+    makes no promise there (its partial sums may or may not overflow depending on how the input is split)."""
+    from spark_rapids_b200 import execs as E
+    big = 6 * 10**37
+    if keyed:
+        b1 = [(1, big), (1, big), (2, 5)] + ([(3, None)] if nullable else [])
+        b2_ = [(1, 1), (2, 7), (3, 4)]
+        want = [(1, None), (2, 12), (3, 4)]
+    else:
+        b1 = [(0, big), (0, big)] + ([(0, None)] if nullable else [])
+        b2_ = [(0, 1)]
+        want = [(None,)]
+    keys = [0] if keyed else []
+    spec = [(b2.AGG_SUM, len(keys), b2.DECIMAL128, 0, 38)]
+    pre = ([b2.col(0, b2.INT64, nullable=False)] if keyed else []) + [b2.col(1, b2.DECIMAL128, 38, 0, nullable=nullable)]
+    src = E.GpuBatchSource(_dec_batches(b2, [b1, b2_], nullable))
+    if plan == "complete":
+        root = E.GpuHashAggregateExec(src, keys, spec, pre_project=pre, mode="complete")
+    else:
+        partial = E.GpuHashAggregateExec(src, keys, spec, pre_project=pre)
+        root = E.GpuHashAggregateExec(E.GpuShuffleExchangeExec(partial, keys), keys, spec, mode="final")
+    out = root.collect()
+    assert out.num_columns == len(keys) + 1
+    assert sorted(out.to_rows(), key=lambda r: r[0] if keyed else 0) == want
+
+
+@pytest.mark.parametrize("plan", ["complete", "partial_exchange_final"])
+def test_nullable_decimal_sum_empty_partials_are_skipped(b2, plan):
+    """keyless SUM over a nullable column whose first batch is all NULL: that partial is empty, not an overflow"""
+    from spark_rapids_b200 import execs as E
+    spec = [(b2.AGG_SUM, 0, b2.DECIMAL128, 0, 38)]
+    pre = [b2.col(1, b2.DECIMAL128, 38, 0, nullable=True)]
+    src = E.GpuBatchSource(_dec_batches(b2, [[(0, None), (0, None)], [(0, 3)], [(0, None)]], True))
+    if plan == "complete":
+        root = E.GpuHashAggregateExec(src, [], spec, pre_project=pre, mode="complete")
+    else:
+        root = E.GpuHashAggregateExec(E.GpuShuffleExchangeExec(E.GpuHashAggregateExec(src, [], spec, pre_project=pre), []), [], spec, mode="final")
+    assert root.collect().to_rows() == [(3,)]
