@@ -259,6 +259,13 @@ int b2_join_probe(b2_handle ht, b2_handle probe_keys_table, int32_t kind,
  * gathered from the unfiltered batch and the filtered copy is never written.  selection = 0: plain b2_join_probe. */
 int b2_join_probe_sel(b2_handle ht, b2_handle probe_keys_table, b2_handle selection, int32_t kind,
                       b2_handle* out_left_map, b2_handle* out_right_map);
+/* INNER join of the rows of `table` that pass `predicate_program` (a GpuFilterExec directly below the stream side).  When
+ * the predicate is a conjunction of NOT NULL integer column-vs-literal comparisons and the build side is distinct on one
+ * NOT NULL 4- or 8-byte integer key of the stream key's dtype, the filter is evaluated inside the probe kernel and no
+ * selection vector exists; otherwise this is b2_filter_row_ids + b2_join_probe_sel.  key_col: the stream key's column in
+ * `table`.  The left map carries ORIGINAL row ids of `table`; out_npass = rows that passed the filter. */
+int b2_join_probe_filter(b2_handle ht, b2_handle table, int32_t key_col, b2_handle predicate_program,
+                         b2_handle* out_left_map, b2_handle* out_right_map, int64_t* out_npass);
 /* Table.gather(map, OutOfBoundsPolicy): out-of-range index -> null row when nullify != 0 */
 int b2_gather(b2_handle table, b2_handle int32_map, int32_t nullify_oob, b2_handle* out_table);
 

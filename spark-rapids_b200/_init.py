@@ -442,6 +442,13 @@ def filter_mask(table, mask):
     return Table(out.value)
 
 
+def filter_row_ids(program, table):
+    """selection vector: INT32 ids (ascending) of the rows that pass"""
+    out = ctypes.c_int64()
+    check(lib.b2_filter_row_ids(program.h, table.h, ctypes.byref(out)))
+    return Column(out.value)
+
+
 def filter_count(program, table):
     out = ctypes.c_int64()
     check(lib.b2_filter_count(program.h, table.h, ctypes.byref(out)))
@@ -528,11 +535,18 @@ class JoinHashTable:
         check(lib.b2_join_build(build_keys.h, int(nulls_equal), ctypes.byref(out)))
         self.h = ctypes.c_int64(out.value)
 
-    def probe(self, probe_keys, kind=JOIN_INNER):
-        """-> (left_map Column, right_map Column|None)"""
+    def probe(self, probe_keys, kind=JOIN_INNER, selection=None):
+        """-> (left_map Column, right_map Column|None); selection: INT32 row ids of probe_keys (filter_row_ids) that take part"""
         lm, rm = ctypes.c_int64(), ctypes.c_int64()
-        check(lib.b2_join_probe(self.h, probe_keys.h, kind, ctypes.byref(lm), ctypes.byref(rm)))
+        check(lib.b2_join_probe_sel(self.h, probe_keys.h, selection.h if selection is not None else 0, kind, ctypes.byref(lm), ctypes.byref(rm)))
         return Column(lm.value), (Column(rm.value) if rm.value else None)
+
+    def probe_filter(self, table, key_col, predicate):
+        """INNER join of the rows of `table` that pass `predicate` (a Program), keyed on column key_col
+        -> (left_map Column of original row ids, right_map Column, rows that passed the filter)"""
+        lm, rm, npass = ctypes.c_int64(), ctypes.c_int64(), ctypes.c_int64()
+        check(lib.b2_join_probe_filter(self.h, table.h, int(key_col), predicate.h, ctypes.byref(lm), ctypes.byref(rm), ctypes.byref(npass)))
+        return Column(lm.value), Column(rm.value), npass.value
 
     def __del__(self):
         if getattr(self, "h", None) is not None and self.h.value:

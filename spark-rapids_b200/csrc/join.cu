@@ -15,6 +15,8 @@
 
 namespace b2 {
 
+Program* program_from(b2_handle h);   // vm.cuh
+
 constexpr uint64_t JSLOT_EMPTY = 0xffffffffffffffffull;
 
 struct JoinTable {
@@ -213,44 +215,91 @@ struct L2Persist {
 
 // The commonest probe of all — INNER join against a distinct build side on ONE integer key column without NULLs (every
 // FK -> PK join of TPC-H) — without the generic row machinery (KeyCols loops, validity, runtime join kind): ~6x fewer
-// instructions per row than join_probe_distinct_kernel.  Each warp takes 256 rows at a time:
-//   1. row ids (through the selection vector), keys, Bloom words: 8 independent loads per lane at each step;
-//   2. the rows that pass the filter (10-20 % in q3) are compacted into a per-warp queue in shared memory, so the random
-//      HBM accesses into the table are issued by FULL warps in one or two rounds (the generic kernel walked its 8 row
+// instructions per row than join_probe_distinct_kernel.  A warp takes PQ x 32 rows at a time (probe_distinct1_rows):
+//   1. keys, then Bloom words: PQ independent loads per lane at each step;
+//   2. the rows that pass the Bloom filter (10-20 % in q3) are compacted into a per-warp queue in shared memory, so the
+//      random HBM accesses into the table are issued by FULL warps in one or two rounds (the generic kernel walked its 8 row
 //      slots one after the other, each round with 2-3 live lanes paying a full memory latency);
-//   3. one output reservation (atomic) per round.
-//   MODE 0: every row of the batch; 1: the rows of a selection vector (a filter below the join emitted row ids);
-//   2: the filter itself is evaluated here (a "simple" predicate, simplefilter.cuh): the predicate columns of the 256 rows are
-//      loaded first, rows that fail are dropped before their key is fetched, and no selection vector is ever written or read.
+//   3. one output reservation (atomic) per round; each round's hits are written in ascending row order when r[] ascends
+//      (j-major, then lane), so the payload gathers read the batch in order.
 // (Tried and measured slower on the q3 step: evict-first loads of the selection vector and the key column plus
 // evict-last Bloom words.  Unlike part_scatter2 — hash.cu — nothing here is half-written and waiting in L2.)
 constexpr int PQ = 8;
-template <typename T>
-__device__ __forceinline__ uint32_t pred_term_mask(const SimpleTerm& t, const int32_t (&r)[PQ]) {
-  T v[PQ];
-#pragma unroll
-  for (int j = 0; j < PQ; j++) v[j] = r[j] >= 0 ? reinterpret_cast<const T*>(t.col)[r[j]] : T(0);
-  const T lit = (T)t.lit;
+template <typename K>
+__device__ __forceinline__ void probe_distinct1_rows(const K* __restrict__ keys, const int32_t (&r)[PQ], const uint64_t* __restrict__ slots,
+                                                     uint32_t mask, const unsigned long long* __restrict__ bloom, uint32_t bloom_mask,
+                                                     unsigned long long* __restrict__ total, int32_t* __restrict__ left_map,
+                                                     int32_t* __restrict__ right_map, int32_t* s_q) {
+  typedef typename std::make_unsigned<K>::type UK;
+  const int lane = threadIdx.x & 31;
+  const uint32_t lt = (1u << lane) - 1u;
   uint32_t pass = 0;
+  if (bloom) {
+    uint32_t h[PQ];
+    unsigned long long wv[PQ];
+#pragma unroll
+    for (int j = 0; j < PQ; j++) h[j] = r[j] >= 0 ? hash_packed((uint64_t)(UK)keys[r[j]]) : 0u;
+#pragma unroll
+    for (int j = 0; j < PQ; j++) {
+      uint32_t wi; unsigned long long bits;
+      bloom_of(h[j], bloom_mask, wi, bits);
+      wv[j] = r[j] >= 0 ? __ldg(&bloom[wi]) : 0ull;
+    }
+#pragma unroll
+    for (int j = 0; j < PQ; j++) {
+      uint32_t wi; unsigned long long bits;
+      bloom_of(h[j], bloom_mask, wi, bits);
+      pass |= (uint32_t)(r[j] >= 0 && (wv[j] & bits) == bits) << j;
+    }
+  } else {
+#pragma unroll
+    for (int j = 0; j < PQ; j++) pass |= (uint32_t)(r[j] >= 0) << j;
+  }
+  int qn = 0;
 #pragma unroll
   for (int j = 0; j < PQ; j++) {
-    const int c = v[j] < lit ? 1 : (v[j] == lit ? 2 : 4);
-    pass |= (uint32_t)((t.truth & c) != 0) << j;
+    const bool p = (pass >> j) & 1u;
+    const uint32_t b = __ballot_sync(0xffffffffu, p);
+    if (p) s_q[qn + __popc(b & lt)] = r[j];
+    qn += __popc(b);
   }
-  return pass;
+  __syncwarp();
+  for (int q0 = 0; q0 < qn; q0 += 32) {
+    const int q = q0 + lane;
+    int32_t br = INT32_MIN, src = 0;
+    if (q < qn) {
+      src = s_q[q];
+      const uint64_t kb = (uint64_t)(UK)keys[src];
+      const uint32_t hh = hash_packed(kb);
+      uint32_t idx = hh & mask;
+      while (true) {
+        const ulonglong2 e = *reinterpret_cast<const ulonglong2*>(&slots[(size_t)idx << 1]);
+        if (e.x == JSLOT_EMPTY) break;
+        if ((uint32_t)(e.x >> 32) == hh && e.y == kb) { br = (int32_t)(uint32_t)e.x; break; }
+        idx = (idx + 1) & mask;
+      }
+    }
+    const bool hit = br != INT32_MIN;
+    const uint32_t b = __ballot_sync(0xffffffffu, hit);
+    if (b) {
+      unsigned long long o = 0;
+      if (lane == 0) o = atomicAdd(total, (unsigned long long)__popc(b));
+      o = __shfl_sync(0xffffffffu, o, 0) + __popc(b & lt);
+      if (hit) { left_map[o] = src; right_map[o] = br; }
+    }
+  }
+  __syncwarp();   // the queue is rewritten by the next call
 }
-template <typename K, int MODE>
+
+// every row of the batch (SEL = false) or the rows of a selection vector (a filter below the join emitted row ids)
+template <typename K, bool SEL>
 __global__ void __launch_bounds__(256) join_probe_distinct1_kernel(const K* __restrict__ keys, const int32_t* __restrict__ sel, int64_t n,
                                                                    const uint64_t* __restrict__ slots, uint32_t mask,
                                                                    const unsigned long long* __restrict__ bloom, uint32_t bloom_mask,
                                                                    unsigned long long* __restrict__ total, int32_t* __restrict__ left_map,
-                                                                   int32_t* __restrict__ right_map, const __grid_constant__ SimplePred sp,
-                                                                   unsigned long long* __restrict__ npass) {
-  constexpr bool SEL = MODE == 1;
-  typedef typename std::make_unsigned<K>::type UK;
-  __shared__ uint8_t s_q[8][32 * PQ];
+                                                                   int32_t* __restrict__ right_map) {
+  __shared__ int32_t s_q[8][32 * PQ];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  const uint32_t lt = (1u << lane) - 1u;
   const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
   for (int64_t base = warp * (32 * PQ); base < n; base += nwarps * (32 * PQ)) {
     int32_t r[PQ];
@@ -259,80 +308,61 @@ __global__ void __launch_bounds__(256) join_probe_distinct1_kernel(const K* __re
       const int64_t rr = base + j * 32 + lane;
       r[j] = rr < n ? (SEL ? sel[rr] : (int32_t)rr) : -1;
     }
-    if (MODE == 2) {   // the filter: PQ independent loads per lane and term
-      uint32_t ok = 0xffu;
-      for (int k = 0; k < sp.n; k++) {
-        const SimpleTerm& t = sp.t[k];
-        switch (t.width) {
-          case 1: ok &= pred_term_mask<int8_t>(t, r); break;
-          case 2: ok &= pred_term_mask<int16_t>(t, r); break;
-          case 4: ok &= pred_term_mask<int32_t>(t, r); break;
-          default: ok &= pred_term_mask<int64_t>(t, r); break;
-        }
-      }
-      int cnt = 0;
-#pragma unroll
-      for (int j = 0; j < PQ; j++) { if (!((ok >> j) & 1u)) r[j] = -1; cnt += r[j] >= 0; }
-      for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
-      if (lane == 0 && cnt) atomicAdd(npass, (unsigned long long)cnt);
-    }
-    uint32_t pass = 0;
-    if (bloom) {
-      uint32_t h[PQ];
-      unsigned long long wv[PQ];
-#pragma unroll
-      for (int j = 0; j < PQ; j++) h[j] = r[j] >= 0 ? hash_packed((uint64_t)(UK)keys[r[j]]) : 0u;
-#pragma unroll
-      for (int j = 0; j < PQ; j++) {
-        uint32_t wi; unsigned long long bits;
-        bloom_of(h[j], bloom_mask, wi, bits);
-        wv[j] = r[j] >= 0 ? __ldg(&bloom[wi]) : 0ull;
-      }
-#pragma unroll
-      for (int j = 0; j < PQ; j++) {
-        uint32_t wi; unsigned long long bits;
-        bloom_of(h[j], bloom_mask, wi, bits);
-        pass |= (uint32_t)(r[j] >= 0 && (wv[j] & bits) == bits) << j;
-      }
-    } else {
-#pragma unroll
-      for (int j = 0; j < PQ; j++) pass |= (uint32_t)(r[j] >= 0) << j;
-    }
+    probe_distinct1_rows<K>(keys, r, slots, mask, bloom, bloom_mask, total, left_map, right_map, s_q[w]);
+  }
+}
+
+// A simple filter (simplefilter.cuh) directly below the stream side, evaluated inside the probe: no selection vector is
+// written, copied back or re-read.  Per tile of FP_TILE consecutive rows:
+//   1. sf_tile streams the predicate columns (16-byte loads, the selection-vector kernel's code) into a bit mask in shared
+//      memory;
+//   2. the passing rows become a dense, ascending queue of tile offsets in shared memory (one mask word per thread, block
+//      scan of the popcounts; the join output is unordered, so no look-back across tiles);
+//   3. full warps take the queue PQ x 32 ids at a time through probe_distinct1_rows.  Lanes only load keys of passing rows:
+//      the same sectors the selection-vector path reads.
+// The probe is bound by latency per row slot, not by bytes, so the queue is what makes the fusion pay: walking every row
+// through the dependent chain (predicate -> key -> Bloom word) would leave the lanes of failing rows idle at every step
+// (about half of them on q3's date filters).  The streaming of one CTA overlaps the lookups of the others (FP_CTAS per SM;
+// 3 measured slower, 5 spills).
+constexpr int FP_TILE = 8 * 1024, FP_WORDS = FP_TILE / 32, FP_CTAS = 4;
+static_assert(FP_WORDS == SF_NT, "one mask word per thread");
+template <typename K>
+__global__ void __launch_bounds__(SF_NT, FP_CTAS) join_filter_probe_kernel(const __grid_constant__ SimplePred sp, const K* __restrict__ keys, int64_t n,
+                                                                          const uint64_t* __restrict__ slots, uint32_t mask,
+                                                                          const unsigned long long* __restrict__ bloom, uint32_t bloom_mask,
+                                                                          unsigned long long* __restrict__ total, int32_t* __restrict__ left_map,
+                                                                          int32_t* __restrict__ right_map, unsigned long long* __restrict__ npass) {
+  __shared__ uint32_t s_mask[FP_WORDS];
+  __shared__ uint16_t s_rows[FP_TILE];               // offsets in the tile of the passing rows, ascending
+  __shared__ int32_t s_q[SF_NT / 32][32 * PQ];
+  __shared__ uint32_t s_wtot[SF_NT / 32];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int64_t ntiles = (n + FP_TILE - 1) / FP_TILE;
+  for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    const int64_t row0 = tile * FP_TILE;
+    sf_tile(sp, row0, (int)min((int64_t)FP_TILE, n - row0), s_mask, FP_WORDS);
+    const uint32_t m = s_mask[threadIdx.x], c = __popc(m);
+    uint32_t inc = c;
+    for (int o = 1; o < 32; o <<= 1) { const uint32_t x = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += x; }
+    if (lane == 31) s_wtot[w] = inc;
+    __syncthreads();
+    uint32_t pos = inc - c;
     int qn = 0;
 #pragma unroll
-    for (int j = 0; j < PQ; j++) {
-      const bool p = (pass >> j) & 1u;
-      const uint32_t b = __ballot_sync(0xffffffffu, p);
-      if (p) s_q[w][qn + __popc(b & lt)] = (uint8_t)(j * 32 + lane);
-      qn += __popc(b);
-    }
-    __syncwarp();
-    for (int q0 = 0; q0 < qn; q0 += 32) {
-      const int q = q0 + lane;
-      int32_t br = INT32_MIN, src = 0;
-      if (q < qn) {
-        const int64_t rr = base + s_q[w][q];
-        src = SEL ? sel[rr] : (int32_t)rr;
-        const uint64_t kb = (uint64_t)(UK)keys[src];
-        const uint32_t hh = hash_packed(kb);
-        uint32_t idx = hh & mask;
-        while (true) {
-          const ulonglong2 e = *reinterpret_cast<const ulonglong2*>(&slots[(size_t)idx << 1]);
-          if (e.x == JSLOT_EMPTY) break;
-          if ((uint32_t)(e.x >> 32) == hh && e.y == kb) { br = (int32_t)(uint32_t)e.x; break; }
-          idx = (idx + 1) & mask;
-        }
+    for (int i = 0; i < SF_NT / 32; i++) { const uint32_t x = s_wtot[i]; pos += i < w ? x : 0u; qn += (int)x; }
+    for (uint32_t mm = m; mm; mm &= mm - 1) s_rows[pos++] = (uint16_t)(threadIdx.x * 32 + __ffs(mm) - 1);
+    if (threadIdx.x == 0 && qn) atomicAdd(npass, (unsigned long long)qn);
+    __syncthreads();
+    for (int q0 = w * 32 * PQ; q0 < qn; q0 += SF_NT * PQ) {
+      int32_t r[PQ];
+#pragma unroll
+      for (int j = 0; j < PQ; j++) {
+        const int q = q0 + j * 32 + lane;
+        r[j] = q < qn ? (int32_t)(row0 + s_rows[q]) : -1;
       }
-      const bool hit = br != INT32_MIN;
-      const uint32_t b = __ballot_sync(0xffffffffu, hit);
-      if (b) {
-        unsigned long long o = 0;
-        if (lane == 0) o = atomicAdd(total, (unsigned long long)__popc(b));
-        o = __shfl_sync(0xffffffffu, o, 0) + __popc(b & lt);
-        if (hit) { left_map[o] = src; right_map[o] = br; }
-      }
+      probe_distinct1_rows<K>(keys, r, slots, mask, bloom, bloom_mask, total, left_map, right_map, s_q[w]);
     }
-    __syncwarp();   // the queue is rewritten by the next chunk
+    __syncthreads();   // s_mask, s_rows and s_wtot are rewritten by the next tile
   }
 }
 
@@ -429,38 +459,35 @@ static JoinTable* jt_from(b2_handle h) {
   return reinterpret_cast<JoinTable*>((intptr_t)h);
 }
 
-// GpuFilter directly below the stream side of an INNER FK -> PK join, fused INTO the probe when the predicate is of the simple
-// shape (simplefilter.cuh) and the probe qualifies for join_probe_distinct1_kernel: the gather maps carry ORIGINAL row ids of
-// `batch`, `npass_out` = rows that passed the filter (the filter node's numOutputRows).  false = not applicable, the caller
-// takes the selection-vector path.
+// GpuFilter directly below the stream side of an INNER FK -> PK join, fused INTO the probe (join_filter_probe_kernel) when
+// the predicate is of the simple shape (simplefilter.cuh) and the probe qualifies for the one-key distinct probe: the gather
+// maps carry ORIGINAL row ids of `batch`, `npass_out` = rows that passed the filter (the filter node's numOutputRows).
+// false = not applicable, the caller takes the selection-vector path (b2_filter_row_ids + b2_join_probe_sel).
 bool join_probe_pred(b2_handle ht, const Table* batch, int key_col, const Program* prog, Column** out_lm, Column** out_rm, int64_t* npass_out) {
-  // OFF by default: measured on the q3 step the fused kernel is slower (the probe took about twice as long).  The probe
-  // is bound by latency per row SLOT, not by bytes, and without the selection vector it walks all 600 M rows with 46 % of
-  // its lanes idle; the filter kernel's compaction is worth more than the 1.3 GB round trip of the row ids.  Kept (and
-  // tested) behind B2_JOIN_PRED_FUSION for a version that compacts the passing rows inside the warp first.
-  if (!getenv("B2_JOIN_PRED_FUSION") || getenv("B2_JOIN_NO_FAST_PROBE")) return false;
+  if (getenv("B2_JOIN_NO_FAST_PROBE")) return false;
   JoinTable* jt = jt_from(ht);
   const int64_t n = batch->rows;
   if (!jt->distinct || !jt->fast || jt->key_idx.size() != 1 || n < (1 << 16) || n >= 0x7fffffffLL) return false;
+  if (key_col < 0 || key_col >= (int)batch->cols.size()) throw Error(B2_ERR_INVALID, "join key index out of range");
   const Column* pc = batch->cols[key_col];
   const int pw = dtype_width(pc->dtype);
   if (pc->nullable() || is_float(pc->dtype) || pc->dtype == B2_STRING || !(pw == 4 || pw == 8)) return false;
   if (pc->dtype != jt->keys->cols[jt->key_idx[0]]->dtype) return false;
   SimplePred sp;
-  if (!simple_pred_of(prog, batch, sp)) return false;
+  if (!simple_pred_of(prog, batch, sp)) return false;   // also: every predicate column 16-byte aligned
   ColGuard lm(new_column(B2_INT32, 0, n, false)), rm(new_column(B2_INT32, 0, n, false));
   DevBuf tot(16);
   CUDA_CHECK(cudaMemsetAsync(tot.p, 0, 16, stream()));
   {
-    KernelTimer kt("join_probe_distinct1_kernel");
-    const int grid = grid_for(n, 256);
+    KernelTimer kt("join_filter_probe_kernel");
+    const int grid = grid_for(n, FP_TILE, FP_CTAS);
     const uint64_t* sl = jt->slots.as<uint64_t>(); const uint32_t msk = (uint32_t)(jt->cap - 1);
     const unsigned long long* bl = jt->bloom.as<unsigned long long>();
     unsigned long long* tp = tot.as<unsigned long long>();
-    if (pw == 8) join_probe_distinct1_kernel<int64_t, 2><<<grid, 256, 0, stream()>>>(pc->data.as<int64_t>(), nullptr, n, sl, msk, bl, jt->bloom_mask, tp,
-                                                                                       lm.c->data.as<int32_t>(), rm.c->data.as<int32_t>(), sp, tp + 1);
-    else join_probe_distinct1_kernel<int32_t, 2><<<grid, 256, 0, stream()>>>(pc->data.as<int32_t>(), nullptr, n, sl, msk, bl, jt->bloom_mask, tp,
-                                                                              lm.c->data.as<int32_t>(), rm.c->data.as<int32_t>(), sp, tp + 1);
+    if (pw == 8) join_filter_probe_kernel<int64_t><<<grid, SF_NT, 0, stream()>>>(sp, pc->data.as<int64_t>(), n, sl, msk, bl, jt->bloom_mask, tp,
+                                                                                 lm.c->data.as<int32_t>(), rm.c->data.as<int32_t>(), tp + 1);
+    else join_filter_probe_kernel<int32_t><<<grid, SF_NT, 0, stream()>>>(sp, pc->data.as<int32_t>(), n, sl, msk, bl, jt->bloom_mask, tp,
+                                                                        lm.c->data.as<int32_t>(), rm.c->data.as<int32_t>(), tp + 1);
     CUDA_CHECK(cudaGetLastError());
     count_launch();
   }
@@ -535,6 +562,29 @@ int b2_join_build(b2_handle build_keys_table, int32_t nulls_equal, b2_handle* ou
 int b2_join_hash_table_close(b2_handle ht) {
   B2_TRY
   delete jt_from(ht);
+  B2_CATCH
+}
+
+int b2_join_probe_filter(b2_handle ht, b2_handle table, int32_t key_col, b2_handle predicate_program, b2_handle* out_left_map,
+                         b2_handle* out_right_map, int64_t* out_npass) {
+  B2_TRY
+  Table* t = table_from(table);
+  B2_CHECK(key_col >= 0 && key_col < (int)t->cols.size(), "join key index out of range");
+  Column* lm = nullptr; Column* rm = nullptr;
+  int64_t npass = 0;
+  if (join_probe_pred(ht, t, key_col, program_from(predicate_program), &lm, &rm, &npass)) {
+    *out_left_map = to_handle(lm); *out_right_map = to_handle(rm); *out_npass = npass;
+    return B2_OK;
+  }
+  b2_handle sel = 0;
+  int rc = b2_filter_row_ids(predicate_program, table, &sel);
+  if (rc != B2_OK) return rc;
+  ColGuard sg(col_from(sel));
+  col_incref(t->cols[key_col]);
+  std::unique_ptr<Table, void (*)(Table*)> keys(new_table({t->cols[key_col]}), table_release);
+  rc = b2_join_probe_sel(ht, to_handle(keys.get()), sel, B2_JOIN_INNER, out_left_map, out_right_map);
+  if (rc != B2_OK) return rc;
+  *out_npass = sg.c->size;
   B2_CATCH
 }
 
@@ -616,13 +666,12 @@ int b2_join_probe_sel(b2_handle ht, b2_handle probe_keys_table, b2_handle select
         const uint64_t* sl = jt->slots.as<uint64_t>(); const uint32_t msk = (uint32_t)(jt->cap - 1);
         const unsigned long long* bl = jt->bloom.as<unsigned long long>(); unsigned long long* tp = tot.as<unsigned long long>();
         int32_t* lp = lm.c->data.as<int32_t>(); int32_t* rp = rm.c->data.as<int32_t>();
-        SimplePred none; memset(&none, 0, sizeof(none));
         if (pw == 8) {
-          if (sel) join_probe_distinct1_kernel<int64_t, 1><<<grid, 256, 0, stream()>>>(pc->data.as<int64_t>(), sel, n, sl, msk, bl, jt->bloom_mask, tp, lp, rp, none, nullptr);
-          else join_probe_distinct1_kernel<int64_t, 0><<<grid, 256, 0, stream()>>>(pc->data.as<int64_t>(), sel, n, sl, msk, bl, jt->bloom_mask, tp, lp, rp, none, nullptr);
+          if (sel) join_probe_distinct1_kernel<int64_t, true><<<grid, 256, 0, stream()>>>(pc->data.as<int64_t>(), sel, n, sl, msk, bl, jt->bloom_mask, tp, lp, rp);
+          else join_probe_distinct1_kernel<int64_t, false><<<grid, 256, 0, stream()>>>(pc->data.as<int64_t>(), sel, n, sl, msk, bl, jt->bloom_mask, tp, lp, rp);
         } else {
-          if (sel) join_probe_distinct1_kernel<int32_t, 1><<<grid, 256, 0, stream()>>>(pc->data.as<int32_t>(), sel, n, sl, msk, bl, jt->bloom_mask, tp, lp, rp, none, nullptr);
-          else join_probe_distinct1_kernel<int32_t, 0><<<grid, 256, 0, stream()>>>(pc->data.as<int32_t>(), sel, n, sl, msk, bl, jt->bloom_mask, tp, lp, rp, none, nullptr);
+          if (sel) join_probe_distinct1_kernel<int32_t, true><<<grid, 256, 0, stream()>>>(pc->data.as<int32_t>(), sel, n, sl, msk, bl, jt->bloom_mask, tp, lp, rp);
+          else join_probe_distinct1_kernel<int32_t, false><<<grid, 256, 0, stream()>>>(pc->data.as<int32_t>(), sel, n, sl, msk, bl, jt->bloom_mask, tp, lp, rp);
         }
         CUDA_CHECK(cudaGetLastError());
         count_launch();

@@ -11,7 +11,7 @@
 
 namespace b2 {
 
-constexpr int SF_NT = 256, SF_WARPS = SF_NT / 32, SF_TILE = 32768, SF_WORDS = SF_TILE / 32, SF_WWORDS = SF_WORDS / SF_WARPS;
+constexpr int SF_WARPS = SF_NT / 32, SF_TILE = 32768, SF_WORDS = SF_TILE / 32, SF_WWORDS = SF_WORDS / SF_WARPS;
 struct SimpleWork { unsigned long long tile_counter, total; };
 
 constexpr uint64_t SLB_AGG = 1ull << 62, SLB_PREFIX = 2ull << 62, SLB_MASK = (1ull << 62) - 1;
@@ -47,31 +47,6 @@ __device__ __forceinline__ int64_t sf_block_lookback(uint64_t* status, int64_t t
   return excl;
 }
 
-// One term over one tile: every thread tests 16-byte vectors of the column, consecutive lanes on consecutive vectors (each
-// warp load covers 512 contiguous bytes; no barrier inside, 4 loads in flight per thread), and clears the bits of the failing
-// rows in the tile's shared bit mask.
-template <typename T>
-__device__ __forceinline__ void sf_term(const SimpleTerm& t, int64_t tile_row0, int tile_n, uint32_t* s_mask) {
-  constexpr int PER = 16 / (int)sizeof(T);                 // rows per vector
-  const uint4* p = reinterpret_cast<const uint4*>(reinterpret_cast<const T*>(t.col) + tile_row0);   // tile_row0 is a multiple of 32768
-  const int nvec = (tile_n + PER - 1) / PER;               // columns are padded to 64 B: a partial last vector is readable, its extra bits are already 0 in the mask
-  const T lit = (T)t.lit;
-#pragma unroll 4
-  for (int v = threadIdx.x; v < nvec; v += SF_NT) {
-    const uint4 w = __ldg(p + v);
-    const T* e = reinterpret_cast<const T*>(&w);
-    uint32_t pass = 0;
-#pragma unroll
-    for (int k = 0; k < PER; k++) {
-      const int c = e[k] < lit ? 1 : (e[k] == lit ? 2 : 4);
-      pass |= (uint32_t)((t.truth & c) != 0) << k;
-    }
-    const uint32_t fail = ~pass & ((1u << PER) - 1u);
-    const int r0 = v * PER;
-    if (fail) atomicAnd(&s_mask[r0 >> 5], ~(fail << (r0 & 31)));
-  }
-}
-
 __global__ void __launch_bounds__(SF_NT) simple_filter_ids_kernel(const __grid_constant__ SimplePred sp, int64_t n, int32_t* __restrict__ ids,
                                                                   uint64_t* __restrict__ status, SimpleWork* __restrict__ work) {
   __shared__ uint32_t s_mask[SF_WORDS];              // bit r: row r of the tile passes every term
@@ -88,21 +63,7 @@ __global__ void __launch_bounds__(SF_NT) simple_filter_ids_kernel(const __grid_c
     if (tile >= ntiles) break;
     const int64_t tile_row0 = tile * SF_TILE;
     const int tile_n = (int)min((int64_t)SF_TILE, n - tile_row0);
-    for (int i = threadIdx.x; i < SF_WORDS; i += SF_NT) {
-      const int lo = i * 32;
-      s_mask[i] = tile_n >= lo + 32 ? 0xffffffffu : (tile_n > lo ? (1u << (tile_n - lo)) - 1u : 0u);
-    }
-    __syncthreads();
-    for (int k = 0; k < sp.n; k++) {
-      const SimpleTerm& t = sp.t[k];
-      switch (t.width) {
-        case 1: sf_term<int8_t>(t, tile_row0, tile_n, s_mask); break;
-        case 2: sf_term<int16_t>(t, tile_row0, tile_n, s_mask); break;
-        case 4: sf_term<int32_t>(t, tile_row0, tile_n, s_mask); break;
-        default: sf_term<int64_t>(t, tile_row0, tile_n, s_mask); break;
-      }
-    }
-    __syncthreads();
+    sf_tile(sp, tile_row0, tile_n, s_mask, SF_WORDS);
     // warp w owns mask words [w * 128, (w + 1) * 128) = rows [w * 4096, (w + 1) * 4096) of the tile
     {
       uint32_t c = 0;
