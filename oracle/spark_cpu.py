@@ -441,7 +441,8 @@ def _cast(a, to):
         return OCol(vals, ok, (tdt, to[1], to[2]))
     if is_decimal(fdt):
         assert tdt in (FLOAT32, FLOAT64)
-        v = np.array([int(x) for x in a.values], dtype=np.float64) / (10.0 ** a.typ[2])
+        # one correctly rounded int -> double, then one division by the double nearest 10^scale (10.0 ** 23 is not)
+        v = np.array([float(int(x)) for x in a.values], dtype=np.float64) / float(10 ** a.typ[2])
         return OCol(v.astype(_NP[tdt]), a.valid, (tdt, 0, 0))
     x = a.values
     if tdt == BOOL8:

@@ -192,11 +192,17 @@ struct Compiler {
     int from_prec = is_decimal(v.dtype) ? v.precision : default_precision(v.dtype);
     if (v.mt == MT_F32 || v.mt == MT_F64) throw Error(B2_ERR_UNSUPPORTED, "float -> decimal cast is not supported");
     if (v.o.kind == OK_LIT && !v.o.lit_null && scale >= from_scale && scale - from_scale <= 18) {
-      // fold literal rescaling at compile time (GpuLiteral arithmetic is constant-folded by Catalyst too)
+      // fold literal rescaling at compile time (GpuLiteral arithmetic is constant-folded by Catalyst too).  A value that
+      // cannot take the next factor of 10 within `precision` digits is out of range: it is not folded, and the
+      // instructions below turn it into NULL at run time.  Checking before each multiply keeps x below 10^38.
       __int128 x = ((__int128)v.o.hi << 64) | (unsigned __int128)(uint64_t)v.o.lo;
-      for (int t = 0; t < scale - from_scale; t++) x *= 10;
       __int128 lim = 1; for (int t = 0; t < precision; t++) lim *= 10;
-      if (x < lim && x > -lim) {
+      bool fits = true;
+      for (int t = 0; t < scale - from_scale && fits; t++) {
+        if (x > lim / 10 || x < -(lim / 10)) fits = false;
+        else x *= 10;
+      }
+      if (fits && x < lim && x > -lim) {
         Val r = v;
         r.o.lo = (int64_t)(uint64_t)x; r.o.hi = (int64_t)(x >> 64);
         r.mt = target_mt; r.dtype = target_dt; r.precision = precision; r.scale = scale;
@@ -214,7 +220,13 @@ struct Compiler {
         cur = emit(V_RESCALE_UP, cur.mt, cur.mt, cur.mt, cur.nullable || may_overflow, ds, &cur, nullptr, nullptr,
                    target_dt, precision, scale);
       }
-      if (cur.mt != target_mt) cur = widen_int(cur, target_mt);
+      if (cur.mt != target_mt) {
+        // narrowing truncates: check the precision on the wide value, before the cast can wrap it into range
+        if (check && precision - scale < from_prec - from_scale)
+          cur = emit(V_CHECK_PREC, cur.mt, cur.mt, cur.mt, true, precision, &cur, nullptr, nullptr, target_dt, precision, scale);
+        check = false;
+        cur = widen_int(cur, target_mt);
+      }
     } else {
       int ds = from_scale - scale;
       cur = emit(V_RESCALE_DOWN, cur.mt, cur.mt, cur.mt, cur.nullable, ds, &cur, nullptr, nullptr, target_dt, precision, scale);
@@ -382,6 +394,35 @@ struct Compiler {
     return emit(op, a.mt, MT_I8, MT_I8, nullable, 0, &a, &b, nullptr, B2_BOOL8, 0, 0);
   }
 
+  // a +- b into DECIMAL(38, rs) when the operands' scales differ.  Rescaling the lower-scale side l first can leave 128
+  // bits while the sum is still in range (|l * 10^ds| near 1.5e38, |h| near -0.9e38).  Instead the higher-scale side is
+  // split as h = hq * 10^ds + hr (HALF_UP, |hr| <= 10^ds / 2) and the sum is (l +- hq) * 10^ds +- hr: l +- hq cannot
+  // overflow, and a product that leaves 128 bits is at least 10^38 away from fitting anyway.
+  Val capped_add_mixed(Val a, Val b, bool sub, int rs) {
+    const bool a_low = a.scale < b.scale;
+    const int ds = rs - std::min(a.scale, b.scale);
+    a = to_decimal(a, 38, a.scale, false); b = to_decimal(b, 38, b.scale, false);
+    if (a.o.kind == OK_LIT) a = emit(V_MOV, MT_I128, MT_I128, MT_I128, a.nullable, 0, &a, nullptr, nullptr, a.dtype, 38, a.scale);
+    if (b.o.kind == OK_LIT) b = emit(V_MOV, MT_I128, MT_I128, MT_I128, b.nullable, 0, &b, nullptr, nullptr, b.dtype, 38, b.scale);
+    Val h = a_low ? b : a, l = a_low ? a : b;
+    auto pin = [&](const Val& v, bool on) { if (v.o.kind == OK_REG) reg_pinned[v.o.idx] = on; };
+    const int D = B2_DECIMAL128, I = MT_I128;
+    pin(h, true);
+    Val hq = emit(V_RESCALE_DOWN, I, I, I, h.nullable, ds, &h, nullptr, nullptr, D, 38, l.scale);
+    pin(hq, true);
+    Val t = emit(V_RESCALE_UP, I, I, I, hq.nullable, ds, &hq, nullptr, nullptr, D, 38, rs);
+    pin(h, false);
+    Val hr = emit(V_SUB, I, I, I, h.nullable || t.nullable, 0, &h, &t, nullptr, D, 38, rs);
+    pin(hq, false);
+    // add: (l + hq) 10^ds + hr;  a - b with a low: (l - hq) 10^ds - hr;  a - b with b low: (hq - l) 10^ds + hr
+    const bool un = l.nullable || hq.nullable;
+    Val u = (sub && !a_low) ? emit(V_SUB, I, I, I, un, 0, &hq, &l, nullptr, D, 38, l.scale)
+                            : emit(sub ? V_SUB : V_ADD, I, I, I, un, 0, &l, &hq, nullptr, D, 38, l.scale);
+    Val w = emit(V_RESCALE_UP, I, I, I, true, ds, &u, nullptr, nullptr, D, 38, rs);
+    Val r = emit(sub && a_low ? V_SUB : V_ADD, I, I, I, true, 0, &w, &hr, nullptr, D, 38, rs);
+    return emit(V_CHECK_PREC, I, I, I, true, 38, &r, nullptr, nullptr, D, 38, rs);
+  }
+
   Val compile_arith(Expr* e) {
     Val a = compile(e->kids[0]), b = compile(e->kids[1]);
     int vop = V_ADD + (e->op - B2_OP_ADD);
@@ -395,8 +436,9 @@ struct Compiler {
         int rp = p, rs = s;
         adjust_precision_scale(rp, rs);
         if (rs != s) throw Error(B2_ERR_UNSUPPORTED, "decimal add with precision loss is not supported");
-        a = to_decimal(a, rp, rs, false); b = to_decimal(b, rp, rs, false);
         bool capped = p > 38;
+        if (capped && s1 != s2) return capped_add_mixed(a, b, e->op == B2_OP_SUB, rs);
+        a = to_decimal(a, rp, rs, false); b = to_decimal(b, rp, rs, false);
         if (a.o.kind == OK_LIT && e->op == B2_OP_ADD) std::swap(a, b);
         if (a.o.kind == OK_LIT) a = emit(V_MOV, a.mt, a.mt, a.mt, a.nullable, 0, &a, nullptr, nullptr, a.dtype, a.precision, a.scale);
         bool nullable = a.nullable || b.nullable || (a.mt == MT_I128 && capped);

@@ -628,21 +628,17 @@ static __device__ __noinline__ void vm_muldec(const TileInfo ti, const RInstr& i
     q[2] = (uint64_t)hi;
     q[3] = (uint64_t)((hi >> 64) + (p11 >> 64));
     if (k > 0) {
-      // divide by 10^k in up to two u64 steps, tracking whether remainder*2 >= 10^k
-      const int k1 = k > 19 ? 19 : k;
-      uint64_t d1 = 1; for (int t = 0; t < k1; t++) d1 *= 10ull;
-      const uint64_t r1 = div256_u64(q, d1);
-      const int k2 = k - k1;
-      bool up;
-      if (k2 > 0) {
-        uint64_t d2 = 1; for (int t = 0; t < k2; t++) d2 *= 10ull;
-        const uint64_t r2 = div256_u64(q, d2);
-        const u128 rem = (u128)r2 * d1 + r1, half = ((u128)d1 * d2) / 2;
-        up = rem >= half;
-      } else {
-        up = (u128)r1 * 2 >= (u128)d1;
+      // divide by 10^k (k <= 39) in u64 steps of at most 19 digits.  Only the last step's remainder r decides HALF_UP:
+      // the whole remainder is r * L + low with low < L (L = product of the earlier divisors), and that last divisor
+      // d = 10^j is even, so  r * L + low >= (d / 2) * L  exactly when  r >= d / 2.
+      uint64_t d = 1, r = 0;
+      for (int left = k; left > 0;) {
+        const int j = left > 19 ? 19 : left;
+        d = 1; for (int t = 0; t < j; t++) d *= 10ull;
+        r = div256_u64(q, d);
+        left -= j;
       }
-      if (up) { for (int t = 0; t < 4; t++) { if (++q[t] != 0) break; } }
+      if (r >= d / 2) { for (int t = 0; t < 4; t++) { if (++q[t] != 0) break; } }
     }
     const u128 mag = ((u128)q[1] << 64) | q[0];
     if (q[2] || q[3] || mag >= p38) v = false;
@@ -680,9 +676,15 @@ static __device__ __noinline__ void vm_divdec(const TileInfo ti, const RInstr& i
   });
 }
 
+// the doubles nearest to 10^0 .. 10^38 (multiplying 10.0s together lands 1 ulp low for 10^25..27, 10^30..32, 10^36..38)
+static __device__ const double kPow10F64[39] = {
+    1e0, 1e1, 1e2, 1e3, 1e4, 1e5, 1e6, 1e7, 1e8, 1e9, 1e10, 1e11, 1e12, 1e13, 1e14, 1e15, 1e16, 1e17, 1e18, 1e19,
+    1e20, 1e21, 1e22, 1e23, 1e24, 1e25, 1e26, 1e27, 1e28, 1e29, 1e30, 1e31, 1e32, 1e33, 1e34, 1e35, 1e36, 1e37, 1e38};
+
+// one correctly rounded integer -> double, then one IEEE division by the correctly rounded 10^scale
 template <typename T>
 __device__ __noinline__ void vm_dec2f64(const TileInfo ti, const RInstr& ins) {
-  double dv = 1.0; for (int t = 0; t < ins.aux; t++) dv *= 10.0;
+  const double dv = kPow10F64[ins.aux];
   vm_loop1<T, double>(ti, ins, [dv](T x, bool&) -> double { return CastVia<T, double>::f(x) / dv; });
 }
 
