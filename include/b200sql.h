@@ -286,6 +286,11 @@ int b2_merge_sorted(const b2_handle* tables, int32_t ntables, const b2_order_by_
 /* Table.lowerBound / upperBound: for each row of `values`, its insertion index in sorted `table` */
 int b2_search_bounds(b2_handle sorted_table, b2_handle values_table, const b2_order_by_arg* keys,
                      int32_t nkeys, int32_t upper, b2_handle* out_int32_idx);
+/* GpuSortExec with the out-of-core sort (GpuSortExec.scala:130-165, GpuOutOfCoreSortIterator :241-630): a stable full sort
+ * of the child's partition that need not fit on the device.  Sorted pieces wait in the spill store and are merged on the GPU;
+ * output batches hold at most target_bytes (data + validity + offsets; raised to 16 KiB; a single row may be larger) and fewer
+ * than 2^31 rows each. */
+int b2_exec_sort_out_of_core(b2_handle child, const b2_order_by_arg* order, int32_t norder, int64_t target_bytes, b2_handle* out);
 
 /* ---- a9: hash partition (HashFunctions.scala:196-209; GpuHashPartitioningBase.scala:36-110;
  *          GpuPartitioning.scala:66-99) ----------------------------------------------------------- */

@@ -186,6 +186,38 @@ JNIEXPORT jlongArray JNICALL Java_ai_rapids_cudf_Table_orderBy(JNIEnv* env, jcla
   return table_to_column_handles(env, out);
 }
 
+/* ---- a8: Table.merge / upperBound / lowerBound, the natives GpuOutOfCoreSortIterator calls through GpuSorter
+ * (SortUtils.scala:172-203 upperBound, :249-301 mergeSortAndCloseWithRetry) ----------------------------------------------------- */
+JNIEXPORT jlongArray JNICALL Java_ai_rapids_cudf_Table_merge(JNIEnv* env, jclass cls, jlongArray j_tables, jintArray j_args) {
+  (void)cls;
+  jsize nt = (*env)->GetArrayLength(env, j_tables), n3 = (*env)->GetArrayLength(env, j_args);
+  jlong* ts = (*env)->GetLongArrayElements(env, j_tables, NULL);
+  jint* a = (*env)->GetIntArrayElements(env, j_args, NULL);
+  b2_handle out = 0;
+  int rc = b2_merge_sorted((const b2_handle*)ts, nt, (const b2_order_by_arg*)a, n3 / 3, &out);
+  (*env)->ReleaseLongArrayElements(env, j_tables, ts, JNI_ABORT);
+  (*env)->ReleaseIntArrayElements(env, j_args, a, JNI_ABORT);
+  if (rc != B2_OK) { b2_throw(env, rc); return NULL; }
+  return table_to_column_handles(env, out);
+}
+static jlong search_bounds(JNIEnv* env, jlong sorted, jlong values, jintArray j_args, int upper) {
+  jsize n3 = (*env)->GetArrayLength(env, j_args);
+  jint* a = (*env)->GetIntArrayElements(env, j_args, NULL);
+  b2_handle out = 0;
+  int rc = b2_search_bounds((b2_handle)sorted, (b2_handle)values, (const b2_order_by_arg*)a, n3 / 3, upper, &out);
+  (*env)->ReleaseIntArrayElements(env, j_args, a, JNI_ABORT);
+  if (rc != B2_OK) { b2_throw(env, rc); return 0; }
+  return (jlong)out;   /* INT32 column of insertion indexes */
+}
+JNIEXPORT jlong JNICALL Java_ai_rapids_cudf_Table_upperBound(JNIEnv* env, jclass cls, jlong sorted, jlong values, jintArray j_args) {
+  (void)cls;
+  return search_bounds(env, sorted, values, j_args, 1);
+}
+JNIEXPORT jlong JNICALL Java_ai_rapids_cudf_Table_lowerBound(JNIEnv* env, jclass cls, jlong sorted, jlong values, jintArray j_args) {
+  (void)cls;
+  return search_bounds(env, sorted, values, j_args, 0);
+}
+
 /* ---- a9: Hash.murmurHash32 (HashFunctions.scala:196-209), Table.partition (GpuHashPartitioningBase.scala:66-80) ------------------ */
 JNIEXPORT jlong JNICALL Java_com_nvidia_spark_rapids_jni_Hash_murmurHash32(JNIEnv* env, jclass cls, jint seed, jlongArray j_cols) {
   (void)cls;

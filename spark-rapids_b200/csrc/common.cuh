@@ -132,6 +132,8 @@ void table_release(Table* t);
 Column* new_column(int dtype, int scale, int64_t size, bool with_validity);
 // make a table taking ownership of the column references
 Table* new_table(std::vector<Column*>&& cols);
+// device bytes of a table as the spill store counts them: data + validity + offsets
+int64_t table_bytes(const Table* t);
 // count nulls from the bitmask into col->null_count, dropping the mask if there are none
 void finalize_nulls(Column* c);
 

@@ -237,7 +237,7 @@ static std::atomic<int64_t> g_spilled_bytes{0}, g_unspilled_bytes{0}, g_retries{
 void note_retry() { g_retries.fetch_add(1); }
 void note_split() { g_splits.fetch_add(1); }
 
-static int64_t table_bytes(const Table* t) {
+int64_t table_bytes(const Table* t) {
   int64_t b = 0;
   for (auto* c : t->cols) b += (int64_t)c->data.bytes + (int64_t)c->valid.bytes + (int64_t)c->offsets.bytes;
   return b;

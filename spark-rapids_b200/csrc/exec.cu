@@ -227,8 +227,9 @@ struct GpuHostBatchSource : GpuExec {
     InFlight f = flight.front(); flight.pop_front();
     CUDA_CHECK(cudaStreamWaitEvent(stream(), f.done, 0));   // the consumer's stream is ordered after the copy; the host does not block
     cudaEventDestroy(f.done);
+    TableRef t(f.t);   // released if the next copy cannot be issued (an OOM under an allocation limit)
     if (next_batch < batches.size() && (int)flight.size() < depth) issue();
-    return f.t;
+    return t.release();
   }
 };
 struct GpuProjectExec : GpuExec {
@@ -660,6 +661,7 @@ struct GpuSortExec : GpuExec {
     if (done) return nullptr;
     done = true;
     TableRef pending;
+    std::vector<TableRef> all;   // full sort: every batch, concatenated once
     while (true) {
       TableRef in(children[0]->next());
       if (!in.t) break;
@@ -669,12 +671,231 @@ struct GpuSortExec : GpuExec {
         if (!pending.t) pending = std::move(top);
         else { std::vector<const Table*> ts{pending.t, top.t}; TableRef cat(concat_tables(ts)); pending = TableRef(sorted(cat.t, limit)); }
       } else {
-        if (!pending.t) pending = std::move(in);
-        else { std::vector<const Table*> ts{pending.t, in.t}; pending = TableRef(concat_tables(ts)); }
+        all.push_back(std::move(in));
       }
     }
-    if (!pending.t) return nullptr;
-    return limit >= 0 ? pending.release() : sorted(pending.t, -1);
+    if (limit >= 0) return pending.release();
+    if (all.empty()) return nullptr;
+    if (all.size() == 1) return sorted(all[0].t, -1);
+    std::vector<const Table*> ts;
+    for (auto& a : all) ts.push_back(a.t);
+    TableRef cat(concat_tables(ts));
+    all.clear();
+    return sorted(cat.t, -1);
+  }
+};
+
+DevBuf merge_runs(const Table* t, const std::vector<int64_t>& off, const b2_order_by_arg* keys, int nkeys, const int64_t* tie);   // sort.cu
+int64_t lower_bound_row(const Table* sorted, const Table* probe, const b2_order_by_arg* keys, int nkeys);
+
+__global__ void ordinal_kernel(int64_t* __restrict__ out, int64_t n, int64_t base) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) out[i] = base + i;
+}
+
+// GpuOutOfCoreSortIterator (GpuSortExec.scala:241-630): a full sort of a partition that need not fit on the device.
+//  1. Every input batch gets an INT64 ordinal column (input position: batch base + row), is sorted (stable, so the ordinal needs
+//     no radix digits) and cut into spillable pieces of at most target/8 bytes.  With the ordinal as the last key the order is
+//     strict: "row x comes before row y" has one answer, which makes the cut below exact and the whole sort stable.
+//  2. A round takes the pending pieces with the smallest first rows (ordered by a device sort of a table of those rows) until
+//     the window would pass the target, merges them (merge_runs), and keeps as final every merged row that sorts before the
+//     first row of the smallest piece left pending (lower_bound_row).  The rest is cut into pieces again.  The window holds the
+//     smallest pending piece and its first row sorts before every other first row, so each round finalises at least one row.
+//  3. Final pieces are concatenated up to the target, and the ordinal is dropped.
+// Every device step runs under with_retry: an OOM spills the idle pieces to the host and tries again.  Output batches are at
+// most `target` bytes as the spill store counts them (table_bytes), unless a single row is larger, and below 2^31 rows.
+struct GpuOutOfCoreSortExec : GpuExec {
+  std::vector<b2_order_by_arg> order;        // the sort keys
+  std::vector<b2_order_by_arg> merge_keys;   // the sort keys, then the ordinal
+  int64_t target = 0;
+  struct Piece {
+    b2_handle sp = 0;
+    int64_t rows = 0, bytes = 0;
+    std::vector<int64_t> chars;    // per column: string bytes
+    std::vector<char> nullable;    // per column: carries validity
+    // pending pieces: their first row, kept on the device outside the spill store (one row per piece, and there are at most
+    // about 8 pieces per target_bytes of input) so that ordering the pieces never brings a spilled piece back
+    TableRef head;
+    Piece() {}
+    Piece(const Piece&) = delete;
+    Piece(Piece&& o) noexcept : sp(o.sp), rows(o.rows), bytes(o.bytes), chars(std::move(o.chars)), nullable(std::move(o.nullable)), head(std::move(o.head)) { o.sp = 0; }
+    Piece& operator=(Piece&& o) noexcept {
+      if (this != &o) { close(); sp = o.sp; o.sp = 0; rows = o.rows; bytes = o.bytes; chars = std::move(o.chars); nullable = std::move(o.nullable); head = std::move(o.head); }
+      return *this;
+    }
+    ~Piece() { close(); }
+    void close() { if (sp) b2_spillable_close(sp); sp = 0; }
+    Table* get() const {
+      b2_handle h = 0;
+      int rc = b2_spillable_get(sp, &h);
+      if (rc != B2_OK) throw Error(rc, b2_last_error());
+      return from_handle_owned(h);
+    }
+  };
+  std::vector<Piece> pending;
+  std::deque<Piece> final_q;
+  int64_t final_bytes = 0, ordinal_base = 0;
+  std::vector<int> dtypes;
+  bool read = false;
+
+  // rows [from, to) of the sorted table `t`, cut into pieces of at most `limit` bytes (a single row may be larger)
+  std::vector<Piece> cut(const Table* t, int64_t from, int64_t to, int64_t limit, bool with_heads) {
+    const int nc = (int)t->cols.size();
+    std::vector<std::vector<int32_t>> offs(nc);   // host copies of the string offsets: piece sizes are exact
+    for (int c = 0; c < nc; c++)
+      if (t->cols[c]->dtype == B2_STRING && to > from) {
+        offs[c].resize((size_t)(to - from + 1));
+        d2h(offs[c].data(), t->cols[c]->offsets.as<int32_t>() + from, offs[c].size());
+      }
+    sync();
+    auto bytes = [&](int64_t s, int64_t e) {
+      const int64_t n = e - s;
+      int64_t b = 0;
+      for (int c = 0; c < nc; c++) {
+        const Column* col = t->cols[c];
+        if (col->dtype == B2_STRING) b += (int64_t)offs[c][e - from] - offs[c][s - from] + (n + 1) * 4;
+        else b += n * dtype_width(col->dtype);
+        if (col->nullable()) b += (int64_t)validity_bytes(n);
+      }
+      return b;
+    };
+    std::vector<Piece> out;
+    for (int64_t s = from; s < to;) {
+      int64_t lo = s + 1, hi = to;   // the largest e in [s+1, to] with bytes(s, e) <= limit, at least s+1
+      while (lo < hi) { const int64_t mid = lo + (hi - lo + 1) / 2; if (bytes(s, mid) <= limit) lo = mid; else hi = mid - 1; }
+      const int64_t e = lo;
+      TableRef piece(slice_table(t, s, e));
+      Piece p;
+      p.rows = e - s; p.bytes = table_bytes(piece.t);
+      for (const Column* c : piece.t->cols) { p.chars.push_back(c->dtype == B2_STRING ? c->chars_bytes : 0); p.nullable.push_back(c->nullable()); }
+      if (with_heads) p.head = TableRef(slice_table(t, s, s + 1));
+      int rc = b2_spillable_create(to_handle(piece.t), &p.sp);
+      if (rc != B2_OK) throw Error(rc, b2_last_error());
+      out.push_back(std::move(p));
+      s = e;
+    }
+    return out;
+  }
+
+  // table_bytes of the concatenation of `n` final pieces without the ordinal
+  int64_t output_bytes(size_t n) const {
+    int64_t rows = 0;
+    for (size_t i = 0; i < n; i++) rows += final_q[i].rows;
+    int64_t b = 0;
+    for (size_t c = 0; c + 1 < dtypes.size(); c++) {
+      bool nullable = false;
+      for (size_t i = 0; i < n; i++) { nullable = nullable || final_q[i].nullable[c]; if (dtypes[c] == B2_STRING) b += final_q[i].chars[c]; }
+      b += dtypes[c] == B2_STRING ? (rows + 1) * 4 : rows * dtype_width(dtypes[c]);
+      if (nullable) b += (int64_t)validity_bytes(rows);
+    }
+    return b;
+  }
+
+  void first_pass() {
+    while (true) {
+      TableRef in(children[0]->next());
+      if (!in.t) break;
+      if (in.t->rows == 0) continue;
+      if (dtypes.empty()) {
+        for (const auto& k : order)   // before the ordinal is appended, which a key one past the last column would name
+          B2_CHECK(k.column >= 0 && k.column < (int)in.t->cols.size(), "sort key column out of range");
+        for (const Column* c : in.t->cols) dtypes.push_back(c->dtype);
+        dtypes.push_back(B2_INT64);
+        merge_keys = order;
+        merge_keys.push_back(b2_order_by_arg{(int32_t)in.t->cols.size(), 1, 1});
+      }
+      std::vector<Piece> pieces = with_retry([&] {
+        ColGuard ord(new_column(B2_INT64, 0, in.t->rows, false));
+        ordinal_kernel<<<grid_for(in.t->rows, 256), 256, 0, stream()>>>(ord.c->data.as<int64_t>(), in.t->rows, ordinal_base);
+        CUDA_CHECK(cudaGetLastError());
+        count_launch();
+        std::vector<Column*> cols(in.t->cols.begin(), in.t->cols.end());
+        for (Column* c : cols) col_incref(c);
+        cols.push_back(ord.release());
+        TableRef with_ord(new_table(std::move(cols)));
+        DevBuf perm = sort_order(with_ord.t, order.data(), (int)order.size());
+        TableRef sorted(gather_table(with_ord.t, perm.as<int32_t>(), with_ord.t->rows, false, nullptr));
+        with_ord.reset();
+        perm.reset();
+        return cut(sorted.t, 0, sorted.t->rows, target / 8, true);
+      });
+      ordinal_base += in.t->rows;
+      for (auto& p : pieces) pending.push_back(std::move(p));
+    }
+  }
+
+  void merge_round() {
+    if (pending.size() > 1) {   // order the pending pieces by their first rows, on the device
+      std::vector<int32_t> rank = with_retry([&] {
+        std::vector<const Table*> hs;
+        for (auto& p : pending) hs.push_back(p.head.t);
+        TableRef heads(concat_tables(hs));
+        DevBuf perm = sort_order(heads.t, merge_keys.data(), (int)merge_keys.size());
+        std::vector<int32_t> h(pending.size());
+        d2h(h.data(), perm.p, h.size());
+        sync();
+        return h;
+      });
+      std::vector<Piece> by_head;
+      for (int32_t r : rank) by_head.push_back(std::move(pending[r]));
+      pending.swap(by_head);
+    }
+    size_t take = 0;
+    int64_t bytes = 0, rows = 0;
+    while (take < pending.size() && (take == 0 || (bytes + pending[take].bytes <= target && rows + pending[take].rows <= 0x7fffffffLL))) {
+      bytes += pending[take].bytes; rows += pending[take].rows; take++;
+    }
+    if (take == pending.size() && take == 1) {   // the last pending piece: final as it stands
+      final_bytes += pending[0].bytes;
+      pending[0].head.reset();
+      final_q.push_back(std::move(pending[0]));
+      pending.clear();
+      return;
+    }
+    std::pair<std::vector<Piece>, std::vector<Piece>> cuts = with_retry([&] {
+      TableRef merged;
+      {
+        std::vector<TableRef> win;
+        std::vector<const Table*> ts;
+        std::vector<int64_t> off{0};
+        for (size_t i = 0; i < take; i++) { win.emplace_back(pending[i].get()); ts.push_back(win.back().t); off.push_back(off.back() + win.back().t->rows); }
+        TableRef cat(concat_tables(ts));
+        win.clear();   // the pieces stay in the spill store (and may leave the device) until the round has succeeded
+        // the ordinal is the tie-break: compared as a plain INT64, not through the normalised key
+        DevBuf perm = merge_runs(cat.t, off, order.data(), (int)order.size(), cat.t->cols.back()->data.as<int64_t>());
+        merged = TableRef(gather_table(cat.t, perm.as<int32_t>(), cat.t->rows, false, nullptr));
+      }
+      const int64_t n = merged.t->rows;
+      const int64_t fin = take == pending.size() ? n : lower_bound_row(merged.t, pending[take].head.t, merge_keys.data(), (int)merge_keys.size());
+      if (fin < 1) throw Error(B2_ERR_INVALID, "out-of-core sort: a merge round finalised no row");
+      return std::make_pair(cut(merged.t, 0, fin, target / 8, false), cut(merged.t, fin, n, target / 8, true));
+    });
+    for (auto& p : cuts.first) { final_bytes += p.bytes; final_q.push_back(std::move(p)); }
+    pending.erase(pending.begin(), pending.begin() + take);
+    for (auto& p : cuts.second) pending.push_back(std::move(p));
+  }
+
+  Table* do_next() override {
+    if (!read) { read = true; first_pass(); }
+    while (!pending.empty() && final_bytes < target) merge_round();
+    if (final_q.empty()) return nullptr;
+    size_t n = 1;
+    int64_t rows = final_q[0].rows;
+    while (n < final_q.size() && rows + final_q[n].rows <= 0x7fffffffLL && output_bytes(n + 1) <= target) rows += final_q[n++].rows;
+    Table* out = with_retry([&] {
+      std::vector<TableRef> parts;
+      for (size_t i = 0; i < n; i++) {
+        TableRef t(final_q[i].get());
+        std::vector<Column*> cols(t.t->cols.begin(), t.t->cols.end() - 1);   // without the ordinal
+        for (Column* c : cols) col_incref(c);
+        parts.emplace_back(new_table(std::move(cols)));
+      }
+      if (n == 1) return parts[0].release();
+      std::vector<const Table*> ts;
+      for (auto& p : parts) ts.push_back(p.t);
+      return concat_tables(ts);
+    });
+    for (size_t i = 0; i < n; i++) { final_bytes -= final_q.front().bytes; final_q.pop_front(); }
+    return out;
   }
 };
 
@@ -981,6 +1202,16 @@ int b2_exec_sort(b2_handle child, const b2_order_by_arg* order, int32_t norder, 
   auto* e = new GpuSortExec();
   e->add_child(exec_from(child));
   e->order.assign(order, order + norder); e->global = global != 0; e->limit = limit;
+  *out = to_handle(e);
+  B2_CATCH
+}
+int b2_exec_sort_out_of_core(b2_handle child, const b2_order_by_arg* order, int32_t norder, int64_t target_bytes, b2_handle* out) {
+  B2_TRY
+  B2_CHECK(norder >= 1 && norder < 16, "out-of-core sort: 1 to 15 sort keys");
+  auto* e = new GpuOutOfCoreSortExec();
+  e->add_child(exec_from(child));
+  e->order.assign(order, order + norder);
+  e->target = std::max<int64_t>(target_bytes, 16 << 10);   // GpuSortExec.targetSize: at least 16 KiB
   *out = to_handle(e);
   B2_CATCH
 }

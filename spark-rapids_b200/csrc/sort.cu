@@ -204,20 +204,23 @@ __device__ __forceinline__ uint32_t norm_byte(const SortCol& c, int64_t row, int
   return c.ascending ? out : (out ^ 255u);
 }
 
-// keys[i] = bytes [8*chunk, 8*chunk+8) of the row key of row perm[i] (byte 8*chunk most significant)
+// bytes [8*chunk, 8*chunk+8) of the row key of `row` (byte 8*chunk most significant)
+__device__ __forceinline__ uint64_t key_chunk(const SortPlan& plan, int64_t row, int chunk) {
+  uint64_t k = 0;
+  const int b0 = chunk * 8;
+  for (int ci = 0; ci < plan.ncols; ci++) {
+    const SortCol& c = plan.c[ci];
+    const int lo = max(b0, c.key_off), hi = min(b0 + 8, c.key_off + c.key_len);
+    for (int b = lo; b < hi; b++) k |= (uint64_t)norm_byte(c, row, b - c.key_off) << (8 * (7 - (b - b0)));
+  }
+  return k;
+}
+
+// keys[i] = chunk `chunk` of the row key of row perm[i]
 __global__ void build_chunk_kernel(const __grid_constant__ SortPlan plan, const int32_t* __restrict__ perm, int64_t n, int chunk,
                                    uint64_t* __restrict__ keys) {
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-    const int64_t row = perm ? perm[i] : i;
-    uint64_t k = 0;
-    const int b0 = chunk * 8;
-    for (int ci = 0; ci < plan.ncols; ci++) {
-      const SortCol& c = plan.c[ci];
-      const int lo = max(b0, c.key_off), hi = min(b0 + 8, c.key_off + c.key_len);
-      for (int b = lo; b < hi; b++) k |= (uint64_t)norm_byte(c, row, b - c.key_off) << (8 * (7 - (b - b0)));
-    }
-    keys[i] = k;
-  }
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+    keys[i] = key_chunk(plan, perm ? perm[i] : i, chunk);
 }
 
 __global__ void max_strlen_kernel(const int32_t* __restrict__ offsets, int64_t n, int32_t* out) {
@@ -228,7 +231,9 @@ __global__ void max_strlen_kernel(const int32_t* __restrict__ offsets, int64_t n
   if ((threadIdx.x & 31) == 0) atomicMax(out, m);
 }
 
-SortPlan make_sort_plan(const Table* t, const b2_order_by_arg* keys, int nkeys, bool force_null_byte = false) {
+// str_max (optional, one entry per key): the padded length of each string key, for plans that must line up with the plans of
+// other tables; otherwise the longest string of the column
+SortPlan make_sort_plan(const Table* t, const b2_order_by_arg* keys, int nkeys, bool force_null_byte = false, const int32_t* str_max = nullptr) {
   B2_CHECK(nkeys >= 1 && nkeys <= SORT_MAX_KEYS, "bad number of sort keys");
   SortPlan p; memset(&p, 0, sizeof(p));
   p.ncols = nkeys;
@@ -242,7 +247,10 @@ SortPlan make_sort_plan(const Table* t, const b2_order_by_arg* keys, int nkeys, 
     c.ascending = keys[k].ascending; c.nulls_first = keys[k].nulls_first;
     c.has_null_byte = (col->nullable() || force_null_byte) ? 1 : 0;
     int vlen = c.width;
-    if (col->dtype == B2_STRING) {
+    if (col->dtype == B2_STRING && str_max) {
+      c.str_max = str_max[k];
+      vlen = c.str_max + 4;
+    } else if (col->dtype == B2_STRING) {
       DevBuf m(4);
       CUDA_CHECK(cudaMemsetAsync(m.p, 0, 4, stream()));
       if (col->size) { max_strlen_kernel<<<grid_for(col->size, 256), 256, 0, stream()>>>(col->offsets.as<int32_t>(), col->size, m.as<int32_t>()); count_launch(); }
@@ -361,6 +369,196 @@ __global__ void bounds_kernel(const __grid_constant__ SortPlan sorted, const __g
 Table* gather_table(const Table* t, const int32_t* d_map, int64_t n, bool nullify_oob, const std::vector<int>* only_cols);
 Table* concat_tables(const std::vector<const Table*>& ts);
 Table* filter_by_mask(const Table* t, Column* m);
+
+// plans of several tables whose normalised keys line up byte for byte: every key column has a null byte and each string key
+// the padding of the longest string over all the tables (bounds_kernel compares two such plans)
+std::vector<SortPlan> shared_sort_plans(const std::vector<const Table*>& ts, const b2_order_by_arg* keys, int nkeys) {
+  std::vector<int32_t> str_max(std::max(nkeys, 1), 0);
+  for (const Table* t : ts) {
+    SortPlan p = make_sort_plan(t, keys, nkeys, true);
+    for (int k = 0; k < nkeys; k++) str_max[k] = std::max(str_max[k], p.c[k].str_max);
+  }
+  std::vector<SortPlan> out;
+  for (const Table* t : ts) out.push_back(make_sort_plan(t, keys, nkeys, true, str_max.data()));
+  return out;
+}
+
+// the first row of `sorted` that does not sort before row 0 of `probe` (both tables hold the key columns `keys` refers to)
+int64_t lower_bound_row(const Table* sorted, const Table* probe, const b2_order_by_arg* keys, int nkeys) {
+  B2_CHECK(probe->rows >= 1, "bounds: empty probe");
+  std::vector<SortPlan> p = shared_sort_plans({sorted, probe}, keys, nkeys);
+  DevBuf out(4);
+  bounds_kernel<<<1, 32, 0, stream()>>>(p[0], p[1], sorted->rows, 1, 0, out.as<int32_t>());
+  CUDA_CHECK(cudaGetLastError());
+  count_launch();
+  int32_t h = 0;
+  d2h(&h, out.p, 1);
+  sync();
+  return h;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Merge of sorted runs (Table.merge, SortUtils.scala:249-301): a tree of pairwise merge-path merges of adjacent runs over the
+// runs' concatenation, producing one gather map.  Rows are compared by the first 8-byte chunk of their normalised key, kept
+// next to the map (8 B per row whatever the key width); only rows whose first chunks are equal compute their further chunks
+// from the columns (key_chunk, the sort's own definition of the order).  On equal keys the left run wins: stable.
+constexpr int MP_NT = 256, MP_ITEMS = 8, MP_TILE = MP_NT * MP_ITEMS;
+
+struct MergeRuns {
+  const uint64_t* keys; const int32_t* rows;   // run A = [a0, a0 + na), run B = [a0 + na, a0 + na + nb) of these arrays
+  int64_t a0, na, nb;
+  uint64_t* keys_out; int32_t* rows_out;       // output [a0, a0 + na + nb); keys_out null on the last level
+};
+
+// tie (optional): a per-row INT64 the caller orders by after the keys (the out-of-core sort's input position), read directly
+// instead of through the normalised key
+__device__ __forceinline__ bool mp_less(const SortPlan& plan, int nchunks, const int64_t* tie, uint64_t ka, int32_t ra, uint64_t kb, int32_t rb) {
+  if (ka != kb) return ka < kb;
+  for (int c = 1; c < nchunks; c++) {
+    const uint64_t x = key_chunk(plan, ra, c), y = key_chunk(plan, rb, c);
+    if (x != y) return x < y;
+  }
+  return tie && tie[ra] < tie[rb];
+}
+
+// number of A rows among the first `d` outputs: the largest i with A[i-1] <= B[d-i] (A wins ties)
+template <typename KA, typename RA>
+__device__ __forceinline__ int64_t mp_search(const SortPlan& plan, int nchunks, const int64_t* tie, KA ak, RA ar, int64_t na, KA bk, RA br, int64_t nb,
+                                             int64_t d) {
+  int64_t lo = max((int64_t)0, d - nb), hi = min(d, na);
+  while (lo < hi) {
+    const int64_t mid = (lo + hi) >> 1;
+    if (!mp_less(plan, nchunks, tie, bk[d - 1 - mid], br[d - 1 - mid], ak[mid], ar[mid])) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo;
+}
+
+// split[t] = A rows before output tile t (t = 0 .. ntiles)
+__global__ void merge_path_partition_kernel(const __grid_constant__ SortPlan plan, int nchunks, const int64_t* __restrict__ tie, MergeRuns m, int64_t ntiles, int64_t* __restrict__ split) {
+  const int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (t > ntiles) return;
+  const int64_t d = min(t * MP_TILE, m.na + m.nb);
+  const uint64_t* ak = m.keys + m.a0; const int32_t* ar = m.rows + m.a0;
+  split[t] = mp_search(plan, nchunks, tie, ak, ar, m.na, ak + m.na, ar + m.na, m.nb, d);
+}
+
+// aligned 16-byte vector stores of the destination for the n elements src[idx[0..n)] in shared memory (scalar head and tail)
+template <typename T>
+__device__ __forceinline__ void mp_store(T* __restrict__ dst, const T* src, const uint16_t* idx, int n) {
+  constexpr int V = 16 / sizeof(T);
+  int head = (int)(((16 - ((uintptr_t)dst & 15)) & 15) / sizeof(T));
+  if (head > n) head = n;
+  for (int i = threadIdx.x; i < head; i += MP_NT) dst[i] = src[idx[i]];
+  const int nvec = (n - head) / V;
+  uint4* dv = reinterpret_cast<uint4*>(dst + head);
+  for (int v = threadIdx.x; v < nvec; v += MP_NT) {
+    union { uint4 u; T e[V]; } w;
+#pragma unroll
+    for (int k = 0; k < V; k++) w.e[k] = src[idx[head + v * V + k]];
+    dv[v] = w.u;
+  }
+  for (int i = head + nvec * V + threadIdx.x; i < n; i += MP_NT) dst[i] = src[idx[i]];
+}
+
+// one CTA per output tile: stage the tile's A and B ranges in shared memory (loads issued in batches of MP_ITEMS per lane),
+// each thread merges MP_ITEMS outputs found by its own merge-path search and notes where each output's row is staged; the
+// tile then leaves as aligned vectors
+__global__ void __launch_bounds__(MP_NT) merge_path_kernel(const __grid_constant__ SortPlan plan, int nchunks, const int64_t* __restrict__ tie, MergeRuns m,
+                                                           const int64_t* __restrict__ split) {
+  __shared__ __align__(16) uint64_t s_key[MP_TILE];
+  __shared__ __align__(16) int32_t s_row[MP_TILE];
+  __shared__ uint16_t s_src[MP_TILE];
+  const int64_t t = blockIdx.x, n = m.na + m.nb;
+  const int64_t d0 = t * MP_TILE, d1 = min(d0 + MP_TILE, n);
+  const int64_t a_lo = split[t], a_hi = split[t + 1];
+  const int64_t b_lo = d0 - a_lo, b_hi = d1 - a_hi;
+  const int na = (int)(a_hi - a_lo), nb = (int)(b_hi - b_lo), cnt = na + nb;
+  {
+    uint64_t k[MP_ITEMS]; int32_t r[MP_ITEMS];
+#pragma unroll
+    for (int i = 0; i < MP_ITEMS; i++) {
+      const int s = i * MP_NT + threadIdx.x;
+      const int64_t g = s < na ? m.a0 + a_lo + s : m.a0 + m.na + b_lo + (s - na);
+      if (s < cnt) { k[i] = m.keys[g]; r[i] = m.rows[g]; }
+    }
+#pragma unroll
+    for (int i = 0; i < MP_ITEMS; i++) {
+      const int s = i * MP_NT + threadIdx.x;
+      if (s < cnt) { s_key[s] = k[i]; s_row[s] = r[i]; }
+    }
+  }
+  __syncthreads();
+  const int diag = min((int)threadIdx.x * MP_ITEMS, cnt);
+  int i = (int)mp_search(plan, nchunks, tie, s_key, s_row, na, s_key + na, s_row + na, nb, diag);
+  int j = diag - i;
+#pragma unroll
+  for (int q = 0; q < MP_ITEMS; q++) {   // s_src[output] = staged position of its row
+    const bool take_a = j >= nb || (i < na && !mp_less(plan, nchunks, tie, s_key[na + j], s_row[na + j], s_key[i], s_row[i]));
+    const int o = diag + q;
+    if (o < cnt) s_src[o] = (uint16_t)(take_a ? i : na + j);
+    if (take_a) i++; else j++;
+  }
+  __syncthreads();
+  mp_store(m.rows_out + m.a0 + d0, s_row, s_src, cnt);
+  if (m.keys_out) mp_store(m.keys_out + m.a0 + d0, s_key, s_src, cnt);
+}
+
+// gather map (int32, t->rows entries) that merges the sorted runs [off[r], off[r+1]) of `t`; rows with equal keys are
+// ordered by tie[row] when `tie` is given (device, t->rows entries), else by run
+DevBuf merge_runs(const Table* t, const std::vector<int64_t>& off, const b2_order_by_arg* keys, int nkeys, const int64_t* tie) {
+  const int64_t n = t->rows;
+  B2_CHECK(!off.empty() && off.front() == 0 && off.back() == n, "merge: run offsets do not cover the table");
+  if (n > 0x7fffffffLL) throw Error(B2_ERR_SIZE_OVERFLOW, "merge of more than 2^31-1 rows");
+  DevBuf rows_a((size_t)std::max<int64_t>(n, 1) * 4);
+  if (n) { iota32_kernel<<<grid_for(n, 256), 256, 0, stream()>>>(rows_a.as<int32_t>(), n); count_launch(); }
+  std::vector<int64_t> runs;   // boundaries of the non-empty runs
+  for (size_t r = 0; r + 1 < off.size(); r++) {
+    B2_CHECK(off[r + 1] >= off[r], "merge: run offsets decrease");
+    if (off[r + 1] > off[r]) runs.push_back(off[r]);
+  }
+  runs.push_back(n);
+  const SortPlan plan = make_sort_plan(t, keys, nkeys, true);   // also checks the keys when there is nothing to merge
+  if (runs.size() <= 2) return rows_a;
+  const int nchunks = (plan.key_bytes + 7) / 8;
+  DevBuf keys_a((size_t)n * 8), keys_b((size_t)n * 8), rows_b((size_t)n * 4);
+  build_chunk_kernel<<<grid_for(n, 256), 256, 0, stream()>>>(plan, nullptr, n, 0, keys_a.as<uint64_t>());
+  CUDA_CHECK(cudaGetLastError());
+  count_launch();
+  DevBuf split((size_t)((n + MP_TILE - 1) / MP_TILE + 2) * 8);
+  while (runs.size() > 2) {
+    const bool last = runs.size() == 3;
+    std::vector<int64_t> next;
+    for (size_t r = 0; r + 1 < runs.size(); r += 2) {
+      next.push_back(runs[r]);
+      if (r + 2 >= runs.size()) {   // odd run out: carried to the next level unchanged
+        const size_t len = (size_t)(runs[r + 1] - runs[r]);
+        CUDA_CHECK(cudaMemcpyAsync(rows_b.as<int32_t>() + runs[r], rows_a.as<int32_t>() + runs[r], len * 4, cudaMemcpyDeviceToDevice, stream()));
+        CUDA_CHECK(cudaMemcpyAsync(keys_b.as<uint64_t>() + runs[r], keys_a.as<uint64_t>() + runs[r], len * 8, cudaMemcpyDeviceToDevice, stream()));
+        continue;
+      }
+      MergeRuns m{keys_a.as<uint64_t>(), rows_a.as<int32_t>(), runs[r], runs[r + 1] - runs[r], runs[r + 2] - runs[r + 1],
+                  last ? nullptr : keys_b.as<uint64_t>(), rows_b.as<int32_t>()};
+      const int64_t ntiles = (m.na + m.nb + MP_TILE - 1) / MP_TILE;
+      {
+        KernelTimer kt("merge_path_partition_kernel");
+        merge_path_partition_kernel<<<(int)((ntiles + 1 + 127) / 128), 128, 0, stream()>>>(plan, nchunks, tie, m, ntiles, split.as<int64_t>());
+        CUDA_CHECK(cudaGetLastError());
+      }
+      {
+        KernelTimer kt("merge_path_kernel");
+        merge_path_kernel<<<(int)ntiles, MP_NT, 0, stream()>>>(plan, nchunks, tie, m, split.as<int64_t>());
+        CUDA_CHECK(cudaGetLastError());
+      }
+      count_launch(2);
+    }
+    next.push_back(n);
+    runs.swap(next);
+    std::swap(rows_a, rows_b);
+    std::swap(keys_a, keys_b);
+  }
+  return rows_a;
+}
 
 // histogram of digit (key >> shift) & 255 over the rows whose key agrees with `pval` on the bits of `pmask`
 __global__ void __launch_bounds__(256) hist_prefix_kernel(const uint64_t* __restrict__ keys, int64_t n, uint64_t pmask, uint64_t pval, int shift,
@@ -488,12 +686,14 @@ int b2_top_n(b2_handle table, const b2_order_by_arg* keys, int32_t nkeys, int64_
 
 int b2_merge_sorted(const b2_handle* tables, int32_t ntables, const b2_order_by_arg* keys, int32_t nkeys, b2_handle* out_table) {
   B2_TRY
-  // Table.merge (SortUtils.scala:301): inputs are sorted; concatenation + stable sort yields a
-  // valid merge (equal keys keep input-table order)
+  // Table.merge (SortUtils.scala:301): the inputs are sorted; the merge-path tree over their concatenation keeps equal keys
+  // in input-table order, as the stable sort of the concatenation would
+  B2_CHECK(ntables >= 1, "merge of zero tables");
   std::vector<const Table*> ts;
-  for (int i = 0; i < ntables; i++) ts.push_back(table_from(tables[i]));
+  std::vector<int64_t> off{0};
+  for (int i = 0; i < ntables; i++) { ts.push_back(table_from(tables[i])); off.push_back(off.back() + ts.back()->rows); }
   std::unique_ptr<Table, void (*)(Table*)> cat(concat_tables(ts), table_release);
-  DevBuf perm = sort_order(cat.get(), keys, nkeys);
+  DevBuf perm = merge_runs(cat.get(), off, keys, nkeys, nullptr);
   *out_table = to_handle(gather_table(cat.get(), perm.as<int32_t>(), cat->rows, false, nullptr));
   B2_CATCH
 }

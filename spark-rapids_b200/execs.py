@@ -160,7 +160,14 @@ def _hash_join(stream_keys, build_keys, join_type, stream, build, nulls_equal, s
                 int(nulls_equal), keep=[stream, build])
 
 
-def GpuSortExec(sort_order, child, global_sort=True):
+def GpuSortExec(sort_order, child, global_sort=True, target_bytes=None):
+    """target_bytes given: the out-of-core full sort (GpuOutOfCoreSortIterator) emitting stable sorted batches of at most
+    target_bytes each (at least 16 KiB) whose input need not fit on the device; otherwise the partition is sorted as one
+    batch (global_sort) or each batch on its own"""
+    if target_bytes is not None:
+        if not global_sort:
+            raise ValueError("target_bytes needs global_sort=True")
+        return _new(lib.b2_exec_sort_out_of_core, child.h, m._order_args(sort_order), len(sort_order), int(target_bytes), keep=[child])
     return _new(lib.b2_exec_sort, child.h, m._order_args(sort_order), len(sort_order), int(global_sort), -1, keep=[child])
 
 
