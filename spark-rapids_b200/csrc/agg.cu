@@ -1398,12 +1398,8 @@ static Table* radix_groupby(const Program* prog, const Table* t, const AggPlan& 
   CUDA_CHECK(cudaMemsetAsync(counter.p, 0, 16, stream()));
   {
     const int vm_smem = prog->hdr.smem_bytes;
-    if (vm_smem > 32 * 1024) CUDA_CHECK(cudaFuncSetAttribute(radix_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, vm_smem));
-    KernelTimer kt("radix_rows_kernel");
-    radix_rows_kernel<<<vm_grid(n, vm_smem, prog->hdr.tile_rows), VM_NT, vm_smem, stream()>>>(prog->d_hdr.as<VMProgramHeader>(), prog->d_code.as<VMInstr>(), in, plan, rp,
-                                                                                                rows_of(A), n, counter.as<unsigned long long>());
-    CUDA_CHECK(cudaGetLastError());
-    count_launch();
+    launch("radix_rows_kernel", radix_rows_kernel, vm_grid(n, vm_smem, prog->hdr.tile_rows), VM_NT, vm_smem, stream(), prog->d_hdr.as<VMProgramHeader>(),
+           prog->d_code.as<VMInstr>(), in, plan, rp, rows_of(A), n, counter.as<unsigned long long>());
   }
   int64_t m = n;
   if (plan.has_pred) { unsigned long long hm = 0; d2h(&hm, counter.p, 1); sync(); m = (int64_t)hm; }
@@ -1431,8 +1427,7 @@ static Table* radix_groupby(const Program* prog, const Table* t, const AggPlan& 
     }
   }
   DevBuf off((size_t)(P + 1) * 4);
-  rg_offsets_kernel<<<grid_for(m, 256), 256, 0, stream()>>>(cur->h.as<uint32_t>(), m, (uint32_t)(P - 1), off.as<int32_t>());
-  count_launch();
+  launch(rg_offsets_kernel, grid_for(m, 256), 256, 0, stream(), cur->h.as<uint32_t>(), m, (uint32_t)(P - 1), off.as<int32_t>());
   // 3. aggregate every partition in shared memory
   DevBuf gk0((size_t)m * 8), gk1(rp.has_k1 ? (size_t)m * 8 : 8), gacc((size_t)m * plan.limbs * 8), gnv((size_t)m * plan.nvalids * 4), ovf(4);
   CUDA_CHECK(cudaMemsetAsync(ovf.p, 0, 4, stream()));
@@ -1440,19 +1435,8 @@ static Table* radix_groupby(const Program* prog, const Table* t, const AggPlan& 
   ap.rows = rows_of(*cur); ap.off = off.as<int32_t>(); ap.P = (int32_t)P; ap.C = C; ap.m = m;
   ap.gk0 = gk0.as<uint64_t>(); ap.gk1 = gk1.as<uint64_t>(); ap.gacc = gacc.as<uint64_t>(); ap.gnvalid = gnv.as<uint32_t>();
   ap.gcount = counter.as<unsigned long long>() + 1; ap.overflow = ovf.as<int32_t>();
-  if (rf) {
-    CUDA_CHECK(cudaFuncSetAttribute(rf->fn, cudaFuncAttributeMaxDynamicSharedMemorySize, agg_smem));
-    KernelTimer kt("radix_agg_fixed_kernel");
-    rf->fn<<<(int)std::min<int64_t>(P, sm_count()), RF_NT, agg_smem, stream()>>>(ap);
-    CUDA_CHECK(cudaGetLastError());
-    count_launch();
-  } else {
-    CUDA_CHECK(cudaFuncSetAttribute(radix_agg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, agg_smem));
-    KernelTimer kt("radix_agg_kernel");
-    radix_agg_kernel<<<(int)std::min<int64_t>(P, sm_count()), RG_NT, agg_smem, stream()>>>(plan, rp, ap);
-    CUDA_CHECK(cudaGetLastError());
-    count_launch();
-  }
+  if (rf) launch("radix_agg_fixed_kernel", rf->fn, (int)std::min<int64_t>(P, sm_count()), RF_NT, agg_smem, stream(), ap);
+  else launch("radix_agg_kernel", radix_agg_kernel, (int)std::min<int64_t>(P, sm_count()), RG_NT, agg_smem, stream(), plan, rp, ap);
   unsigned long long hg = 0; int32_t hovf = 0;
   d2h(&hg, counter.as<unsigned long long>() + 1, 1);
   d2h(&hovf, ovf.p, 1);
@@ -1470,11 +1454,9 @@ static Table* radix_groupby(const Program* prog, const Table* t, const AggPlan& 
   }
   AggOut ao;
   make_agg_outputs(plan, prog, specs, naggs, ngroups, outs, ao);
-  if (ngroups) {
-    radix_finalize_kernel<<<grid_for(ngroups, 256), 256, 0, stream()>>>(plan, rp, ngroups, gk0.as<uint64_t>(), gk1.as<uint64_t>(), gacc.as<uint64_t>(), gnv.as<uint32_t>(), ao, ko);
-    CUDA_CHECK(cudaGetLastError());
-    count_launch();
-  }
+  if (ngroups)
+    launch(radix_finalize_kernel, grid_for(ngroups, 256), 256, 0, stream(), plan, rp, ngroups, gk0.as<uint64_t>(), gk1.as<uint64_t>(), gacc.as<uint64_t>(),
+           gnv.as<uint32_t>(), ao, ko);
   sync();   // the scratch arrays are freed on return
   return new_table(outs.release());
 }
@@ -1561,8 +1543,7 @@ Table* scan_aggregate(const Program* prog, bool has_pred, const Table* t, const 
     gt.slots = slots.as<int32_t>(); gt.acc = acc.as<uint64_t>(); gt.nvalid = nv.as<uint32_t>(); gt.mask = (uint32_t)(cap - 1);
     gt.overflow = ovf.as<int32_t>();
     CUDA_CHECK(cudaMemsetAsync(ovf.p, 0, 4, stream()));
-    init_table_kernel<<<grid_for(cap, 256), 256, 0, stream()>>>(gt, plan, cap);
-    count_launch();
+    launch(init_table_kernel, grid_for(cap, 256), 256, 0, stream(), gt, plan, cap);
   };
 
   DevBuf slots, acc, nv, ovf;
@@ -1586,11 +1567,8 @@ Table* scan_aggregate(const Program* prog, bool has_pred, const Table* t, const 
       int64_t pcap = 1;
       while (pcap < (int64_t)grid * nslots * 2) pcap <<= 1;
       alloc_table(pcap, ps, pa, pn, po, pg);
-      if (smem > 32 * 1024) CUDA_CHECK(cudaFuncSetAttribute(aggregate_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-      aggregate_kernel<true><<<grid, VM_NT, smem, stream()>>>(prog->d_hdr.as<VMProgramHeader>(), prog->d_code.as<VMInstr>(), in, plan, pg, pn_rows,
-                                                                (vm_smem + 15) & ~15);
-      CUDA_CHECK(cudaGetLastError());
-      count_launch();
+      launch(aggregate_kernel<true>, grid, VM_NT, smem, stream(), prog->d_hdr.as<VMProgramHeader>(), prog->d_code.as<VMInstr>(), in, plan, pg, pn_rows,
+             (vm_smem + 15) & ~15);
       int32_t h = 0;
       d2h(&h, po.p, 1);
       sync();
@@ -1618,14 +1596,9 @@ Table* scan_aggregate(const Program* prog, bool has_pred, const Table* t, const 
       while (cap < (int64_t)grid * nslots * 2) cap <<= 1;
       if (nkeys == 0) cap = 1;
       alloc_table(cap, slots, acc, nv, ovf, gt);
-      if (n > 0 || nkeys == 0) {
-        if (smem > 32 * 1024) CUDA_CHECK(cudaFuncSetAttribute(aggregate_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        KernelTimer kt_aggregate_smem_kernel("aggregate_smem_kernel");
-        aggregate_kernel<true><<<grid, VM_NT, smem, stream()>>>(prog->d_hdr.as<VMProgramHeader>(), prog->d_code.as<VMInstr>(), in, plan, gt, n,
-                                                                  (vm_smem + 15) & ~15);
-        CUDA_CHECK(cudaGetLastError());
-        count_launch();
-      }
+      if (n > 0 || nkeys == 0)
+        launch("aggregate_smem_kernel", aggregate_kernel<true>, grid, VM_NT, smem, stream(), prog->d_hdr.as<VMProgramHeader>(), prog->d_code.as<VMInstr>(), in,
+               plan, gt, n, (vm_smem + 15) & ~15);
       int32_t h_ovf = 0;
       if (nkeys > 0) { d2h(&h_ovf, ovf.p, 1); sync(); }
       done = h_ovf == 0;
@@ -1635,17 +1608,12 @@ Table* scan_aggregate(const Program* prog, bool has_pred, const Table* t, const 
     cap = 1024;
     while (cap < n * 2) cap <<= 1;
     alloc_table(cap, slots, acc, nv, ovf, gt);
-    if (vm_smem > 32 * 1024) CUDA_CHECK(cudaFuncSetAttribute(aggregate_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, vm_smem));
-    KernelTimer kt_aggregate_global_kernel("aggregate_global_kernel");
-    aggregate_kernel<false><<<vm_grid(n, vm_smem, prog->hdr.tile_rows), VM_NT, vm_smem, stream()>>>(prog->d_hdr.as<VMProgramHeader>(), prog->d_code.as<VMInstr>(), in,
-                                                                                plan, gt, n, (vm_smem + 15) & ~15);
-    CUDA_CHECK(cudaGetLastError());
-    count_launch();
+    launch("aggregate_global_kernel", aggregate_kernel<false>, vm_grid(n, vm_smem, prog->hdr.tile_rows), VM_NT, vm_smem, stream(),
+           prog->d_hdr.as<VMProgramHeader>(), prog->d_code.as<VMInstr>(), in, plan, gt, n, (vm_smem + 15) & ~15);
   }
   // compact occupied slots
   DevBuf pos((size_t)(cap + 1) * 4);
-  occupied_flags_kernel<<<grid_for(cap, 256), 256, 0, stream()>>>(gt.slots, cap, pos.as<int32_t>());
-  count_launch();
+  launch(occupied_flags_kernel, grid_for(cap, 256), 256, 0, stream(), gt.slots, cap, pos.as<int32_t>());
   DevBuf sums = exclusive_scan<int32_t, int32_t>(pos.as<int32_t>(), pos.as<int32_t>(), cap, true);
   int32_t ngroups = 0;
   d2h(&ngroups, pos.as<int32_t>() + cap, 1);
@@ -1654,9 +1622,7 @@ Table* scan_aggregate(const Program* prog, bool has_pred, const Table* t, const 
   AggOut ao;
   make_agg_outputs(plan, prog, specs, naggs, ngroups, outs, ao);
   DevBuf rep((size_t)std::max(ngroups, 1) * 4);
-  finalize_kernel<<<grid_for(cap, 256), 256, 0, stream()>>>(gt, plan, cap, pos.as<int32_t>(), ao, rep.as<int32_t>());
-  CUDA_CHECK(cudaGetLastError());
-  count_launch();
+  launch(finalize_kernel, grid_for(cap, 256), 256, 0, stream(), gt, plan, cap, pos.as<int32_t>(), ao, rep.as<int32_t>());
   std::vector<Column*> result;
   if (nkeys > 0) {
     Table* kt = gather_table(t, rep.as<int32_t>(), ngroups, false, &key_table_cols);

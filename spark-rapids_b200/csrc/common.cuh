@@ -8,6 +8,7 @@
 #include <memory>
 #include <stdexcept>
 #include <string>
+#include <utility>
 #include <vector>
 #include "../../include/b200sql.h"
 
@@ -43,8 +44,8 @@ void cuda_check(cudaError_t e, const char* what, const char* file, int line);
 cudaStream_t stream();
 void* dev_alloc(size_t bytes);            // throws Error(B2_ERR_OOM)
 void dev_free(void* p);
-void count_launch(int n = 1);
-struct KernelTimer {  // scoped CUDA-event timer around a kernel launch; no-op unless profiling is on
+void count_launch();
+struct KernelTimer {  // scoped CUDA-event timer around a kernel launch; no-op unless profiling is on, or without a name
   void* rec;
   cudaStream_t st;
   explicit KernelTimer(const char* name, cudaStream_t on = nullptr);
@@ -194,6 +195,27 @@ __device__ __forceinline__ bool bit_get(const uint32_t* m, int64_t i) {
 }
 __device__ __forceinline__ bool row_valid(const uint32_t* m, int64_t i) {
   return m == nullptr || bit_get(m, i);
+}
+
+// Every kernel launch of the library goes through launch(), so each one is checked and counted the same way.
+// A launch asking for more dynamic shared memory than the kernel's limit first raises the limit (core.cu).
+void reserve_dyn_smem(const void* kernel, size_t smem);
+// Raises a rejected launch as an Error naming the kernel; counts the launch otherwise (core.cu).
+void launch_done(const void* kernel);
+
+// Named form: `timer` (may be null) times exactly this launch when profiling is on.
+template <typename... P, typename... A>
+inline void launch(const char* timer, void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, A&&... args) {
+  if (smem) reserve_dyn_smem((const void*)kernel, smem);
+  {
+    KernelTimer kt(timer, st);
+    kernel<<<grid, block, smem, st>>>(std::forward<A>(args)...);
+  }
+  launch_done((const void*)kernel);
+}
+template <typename... P, typename... A>
+inline void launch(void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, A&&... args) {
+  launch(nullptr, kernel, grid, block, smem, st, std::forward<A>(args)...);
 }
 typedef __int128 i128;
 typedef unsigned __int128 u128;

@@ -8,6 +8,8 @@
 #include <algorithm>
 #include <unordered_map>
 #include <cstdio>
+#include <cstdlib>
+#include <cxxabi.h>
 #include "common.cuh"
 
 namespace b2 {
@@ -60,14 +62,14 @@ static std::unordered_map<void*, size_t> g_sizes;
 static thread_local cudaStream_t t_stream = nullptr;
 static thread_local bool t_stream_owned = false;
 
-void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
+void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
 
 struct ProfRec { const char* name; cudaEvent_t a, b; };
 static std::atomic<bool> g_prof{false};
 static std::mutex g_prof_mu;
 static std::vector<ProfRec*> g_prof_recs;
 KernelTimer::KernelTimer(const char* name, cudaStream_t on) : rec(nullptr), st(on) {
-  if (!g_prof.load(std::memory_order_relaxed)) return;
+  if (!name || !g_prof.load(std::memory_order_relaxed)) return;
   if (!st) st = stream();
   ProfRec* r = new ProfRec();
   r->name = name;
@@ -82,6 +84,44 @@ KernelTimer::~KernelTimer() {
   std::lock_guard<std::mutex> lk(g_prof_mu);
   g_prof_recs.push_back(r);
 }
+// The limit is per kernel and only ever raised, under one lock, so a thread launching with less shared memory
+// can never lower it between another thread's raise and launch.  A kernel starts out allowed 48 KB of shared
+// memory in all, static included; the first launch with dynamic shared memory reads both once.
+void reserve_dyn_smem(const void* kernel, size_t smem) {
+  static std::mutex mu;
+  static std::unordered_map<const void*, size_t> limit;   // kernel -> dynamic shared memory it may launch with
+  std::lock_guard<std::mutex> lk(mu);
+  auto it = limit.find(kernel);
+  if (it == limit.end()) {
+    cudaFuncAttributes a;
+    CUDA_CHECK(cudaFuncGetAttributes(&a, kernel));
+    const size_t dflt = a.sharedSizeBytes < 48 * 1024 ? 48 * 1024 - a.sharedSizeBytes : 0;
+    it = limit.emplace(kernel, std::min<size_t>(dflt, (size_t)a.maxDynamicSharedSizeBytes)).first;
+  }
+  if (smem <= it->second) return;
+  CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  it->second = smem;
+}
+
+void launch_done(const void* kernel) {
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) {
+    std::string what = "launch of ";
+    const char* name = nullptr;
+    if (cudaFuncGetName(&name, kernel) == cudaSuccess && name) {
+      int st = 0;
+      char* dm = abi::__cxa_demangle(name, nullptr, nullptr, &st);
+      what += st == 0 && dm ? dm : name;
+      free(dm);
+    } else {
+      cudaGetLastError();   // the failed lookup must not surface at a later, unrelated check
+      what += "a kernel";
+    }
+    cuda_check(e, what.c_str(), __FILE__, __LINE__);
+  }
+  count_launch();
+}
+
 int sm_count() { return g_sms; }
 bool profile_enabled() { return g_prof.load(std::memory_order_relaxed); }
 
@@ -164,9 +204,7 @@ void h2d_bytes(void* dst, const void* src, size_t bytes) {
   r.head = at + need;
   const int threads = 256;
   const int blocks = (int)std::min<size_t>(64, (bytes / 16 + threads - 1) / threads + 1);
-  KernelTimer kt_stage_pull("stage_pull_kernel");
-  stage_pull_kernel<<<blocks, threads, 0, s>>>((char*)dst, r.dev + at, bytes);
-  CUDA_CHECK(cudaGetLastError());
+  launch("stage_pull_kernel", stage_pull_kernel, blocks, threads, 0, s, (char*)dst, r.dev + at, bytes);
 }
 
 int64_t spill_device(int64_t want_bytes);   // below: the spill store
@@ -379,8 +417,7 @@ static int64_t count_nulls(Column* c) {
   DevBuf cnt(8);
   CUDA_CHECK(cudaMemsetAsync(cnt.p, 0, 8, stream()));
   int64_t words = (c->size + 31) >> 5;
-  count_valid_kernel<<<grid_for(words, 256), 256, 0, stream()>>>(c->validity(), c->size, cnt.as<unsigned long long>());
-  count_launch();
+  launch(count_valid_kernel, grid_for(words, 256), 256, 0, stream(), c->validity(), c->size, cnt.as<unsigned long long>());
   unsigned long long h = 0;
   d2h(&h, cnt.p, 1);
   sync();
@@ -555,10 +592,7 @@ int b2_column_from_scalar(int32_t dtype, int32_t scale, int64_t size, const void
   ColGuard g(new_column(dtype, scale, size, !is_valid));
   uint4 v = {0, 0, 0, 0};
   if (value16) memcpy(&v, value16, 16);
-  if (size) {
-    fill_kernel<<<grid_for(size, 256), 256, 0, stream()>>>(g.c->data.as<uint8_t>(), size, dtype_width(dtype), v);
-    count_launch();
-  }
+  if (size) launch(fill_kernel, grid_for(size, 256), 256, 0, stream(), g.c->data.as<uint8_t>(), size, dtype_width(dtype), v);
   if (!is_valid) {
     CUDA_CHECK(cudaMemsetAsync(g.c->valid.p, 0, g.c->valid.bytes, stream()));
     g.c->null_count = size;

@@ -74,6 +74,8 @@ static void nccl_check(ncclResult_t r, const char* what) {
   if (r != ncclSuccess) throw Error(B2_ERR_CUDA, std::string(what) + ": " + g_nccl.GetErrorString(r));
 }
 #define NCCL_CHECK(x) nccl_check((x), #x)
+// an NCCL collective or group that b2_kernel_launch_count counts as one launch (it enqueues one NCCL kernel)
+#define NCCL_LAUNCH(x) do { NCCL_CHECK(x); count_launch(); } while (0)
 
 constexpr int XMAX_W = 16;      // ranks of one NVSwitch domain
 constexpr int XMAX_COLS = 32;   // columns of an exchanged table on the fused path
@@ -501,8 +503,7 @@ int b2_comm_allmax(b2_handle h, int32_t value, int32_t* out) {
   cudaStream_t s = stream();
   DevBuf a(4), b(4 * (size_t)c->world);
   h2d_bytes(a.p, &value, 4);
-  NCCL_CHECK(g_nccl.AllGather(a.p, b.p, 4, ncclInt8, c->comm, s));
-  count_launch();
+  NCCL_LAUNCH(g_nccl.AllGather(a.p, b.p, 4, ncclInt8, c->comm, s));
   std::vector<int32_t> all(c->world);
   CUDA_CHECK(cudaMemcpyAsync(all.data(), b.p, 4 * (size_t)c->world, cudaMemcpyDeviceToHost, s));
   CUDA_CHECK(cudaStreamSynchronize(s));
@@ -622,20 +623,15 @@ int b2_exchange_hash_sel(b2_handle comm, b2_handle table, b2_handle selection, c
         else if (dt == B2_INT32 || dt == B2_DATE32) km = 2;
       }
       auto kern = km == 1 ? xchg_scatter_kernel<1> : (km == 2 ? xchg_scatter_kernel<2> : xchg_scatter_kernel<0>);
-      if (smem > 40 * 1024) CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
       const int64_t ntiles = (nsend + XS_TILE - 1) / XS_TILE;
       const int per_sm = std::max(1, std::min(3, (200 * 1024) / (smem + 2048)));
       const int grid = (int)std::min<int64_t>(ntiles, (int64_t)sm_count() * per_sm);
-      KernelTimer kt("xchg_scatter_kernel");
-      kern<<<grid, XS_NT, smem, s>>>(keys, pl, nsend, (uint32_t)seed, c->d_hdr->counts);
-      CUDA_CHECK(cudaGetLastError());
-      count_launch();
+      launch("xchg_scatter_kernel", kern, grid, XS_NT, smem, s, keys, pl, nsend, (uint32_t)seed, c->d_hdr->counts);
     }
     {
       // sizes + schema + has-data of every rank; also the completion barrier of every rank's peer stores
       KernelTimer kt("xchg_header_allgather");
-      NCCL_CHECK(g_nccl.AllGather(c->d_hdr, c->d_all, sizeof(XHeader), ncclInt8, c->comm, s));
-      count_launch();
+      NCCL_LAUNCH(g_nccl.AllGather(c->d_hdr, c->d_all, sizeof(XHeader), ncclInt8, c->comm, s));
     }
     CUDA_CHECK(cudaMemcpyAsync(c->h_all, c->d_all, sizeof(XHeader) * W, cudaMemcpyDeviceToHost, s));
     CUDA_CHECK(cudaStreamSynchronize(s));
@@ -708,8 +704,7 @@ int b2_exchange_hash_sel(b2_handle comm, b2_handle table, b2_handle selection, c
         biggest = std::max(biggest, cnt * widths[i]);
         if (oc->valid.p) {
           const uint8_t* vb = ((all[r].nullable_mask >> i) & 1u) ? reinterpret_cast<const uint8_t*>(region + L.val_off[i]) : nullptr;
-          bytes_to_bits_at_kernel<<<grid_for(cnt, 256), 256, 0, s>>>(vb, cnt, oc->valid.as<uint32_t>(), row);
-          count_launch();
+          launch(bytes_to_bits_at_kernel, grid_for(cnt, 256), 256, 0, s, vb, cnt, oc->valid.as<uint32_t>(), row);
         }
       }
       row += cnt;
@@ -719,12 +714,9 @@ int b2_exchange_hash_sel(b2_handle comm, b2_handle table, b2_handle selection, c
       h2d_bytes(d_segs.p, segs.data(), segs.size() * sizeof(CopySeg));
       const int gx = (int)std::max<int64_t>(1, std::min<int64_t>((biggest / 16 + 255) / 256, (int64_t)sm_count() * 4));
       const int gy = (int)std::min<size_t>(segs.size(), 64);
-      xchg_copy_out_kernel<<<dim3(gx, gy), 256, 0, s>>>(d_segs.as<CopySeg>(), (int)segs.size());
-      count_launch();
-      CUDA_CHECK(cudaGetLastError());
+      launch(xchg_copy_out_kernel, dim3(gx, gy), 256, 0, s, d_segs.as<CopySeg>(), (int)segs.size());
       // d_segs is stream-ordered: freed after the kernel
     }
-    CUDA_CHECK(cudaGetLastError());
   }
   if (t) for (int d = 0; d < W; d++) if (d != me) c->bytes_sent += (int64_t)all[me].counts[d] * row_bytes;
   for (int r = 0; r < W; r++) if (r != me) c->bytes_received += (int64_t)all[r].counts[me] * row_bytes;
@@ -755,8 +747,7 @@ int b2_exchange_ex(b2_handle comm, b2_handle partitioned_table, const int32_t* o
   for (int i = 0; i < hdr.ncols; i++) { hdr.dtype[i] = c->schema_dtype[i]; hdr.scale[i] = c->schema_scale[i]; }
   if (t) for (int i = 0; i < hdr.ncols; i++) if (t->cols[i]->nullable()) hdr.nullable_mask |= 1u << i;
   h2d_bytes(c->d_hdr, &hdr, sizeof(hdr));
-  NCCL_CHECK(g_nccl.AllGather(c->d_hdr, c->d_all, sizeof(XHeader), ncclInt8, c->comm, s));
-  count_launch();
+  NCCL_LAUNCH(g_nccl.AllGather(c->d_hdr, c->d_all, sizeof(XHeader), ncclInt8, c->comm, s));
   CUDA_CHECK(cudaMemcpyAsync(c->h_all, c->d_all, sizeof(XHeader) * W, cudaMemcpyDeviceToHost, s));
   // char offsets of the string columns at the partition boundaries ride the same sync
   std::vector<int> str_cols;
@@ -831,7 +822,7 @@ int b2_exchange_ex(b2_handle comm, b2_handle partitioned_table, const int32_t* o
       oc->valid = DevBuf(validity_bytes(out_rows)); oc->null_count = -1;
       temps.emplace_back((size_t)std::max<int64_t>(t->rows, 1));
       uint8_t* sv = temps.back().as<uint8_t>();
-      if (t->rows) { bits_to_bytes_kernel<<<grid_for(t->rows, 256), 256, 0, s>>>(ic->validity(), t->rows, sv); count_launch(); }
+      if (t->rows) launch(bits_to_bytes_kernel, grid_for(t->rows, 256), 256, 0, s, ic->validity(), t->rows, sv);
       temps.emplace_back((size_t)std::max<int64_t>(out_rows, 1));
       uint8_t* rv = temps.back().as<uint8_t>();
       row_xfer(sv, rv, 1);
@@ -841,7 +832,7 @@ int b2_exchange_ex(b2_handle comm, b2_handle partitioned_table, const int32_t* o
     if (ic->dtype == B2_STRING) {
       temps.emplace_back((size_t)std::max<int64_t>(t->rows, 1) * 4);
       int32_t* slen = temps.back().as<int32_t>();
-      if (t->rows) { lengths_kernel<<<grid_for(t->rows, 256), 256, 0, s>>>(ic->offsets.as<int32_t>(), t->rows, slen); count_launch(); }
+      if (t->rows) launch(lengths_kernel, grid_for(t->rows, 256), 256, 0, s, ic->offsets.as<int32_t>(), t->rows, slen);
       temps.emplace_back((size_t)(out_rows + 1) * 4);
       int32_t* rlen = temps.back().as<int32_t>();
       row_xfer(slen, rlen, 4);
@@ -880,11 +871,10 @@ int b2_exchange_ex(b2_handle comm, b2_handle partitioned_table, const int32_t* o
         if (r != me) { c->bytes_sent += sb; c->bytes_received += rb; }
       }
     }
-    NCCL_CHECK(g_nccl.GroupEnd());
-    count_launch();
+    NCCL_LAUNCH(g_nccl.GroupEnd());
   }
   for (auto& vf : valid_fix) {
-    if (out_rows) { bytes_to_bits_kernel<<<grid_for(out_rows, 256), 256, 0, s>>>(vf.second, out_rows, vf.first->valid.as<uint32_t>()); count_launch(); }
+    if (out_rows) launch(bytes_to_bits_kernel, grid_for(out_rows, 256), 256, 0, s, vf.second, out_rows, vf.first->valid.as<uint32_t>());
   }
   for (auto& sf : str_fix) exclusive_scan<int32_t, int32_t>(sf.second, sf.first->offsets.as<int32_t>(), out_rows, true);
   sync();  // temps are freed on return
@@ -921,8 +911,7 @@ int b2_broadcast_table(b2_handle comm, b2_handle table, int32_t root, b2_handle*
   }
   DevBuf d_bh(sizeof(BHeader));
   if (t) h2d_bytes(d_bh.p, &bh, sizeof(bh));
-  NCCL_CHECK(g_nccl.Broadcast(d_bh.p, d_bh.p, sizeof(BHeader), ncclInt8, root, c->comm, s));
-  count_launch();
+  NCCL_LAUNCH(g_nccl.Broadcast(d_bh.p, d_bh.p, sizeof(BHeader), ncclInt8, root, c->comm, s));
   CUDA_CHECK(cudaMemcpyAsync(&bh, d_bh.p, sizeof(bh), cudaMemcpyDeviceToHost, s));
   CUDA_CHECK(cudaStreamSynchronize(s));
   if (me == root) { t->refs.fetch_add(1); }
@@ -948,8 +937,7 @@ int b2_broadcast_table(b2_handle comm, b2_handle table, int32_t root, b2_handle*
     }
     if ((bh.nullable_mask >> i) & 1u) NCCL_CHECK(g_nccl.Broadcast(oc->valid.p, oc->valid.p, validity_bytes(bh.rows), ncclInt8, root, c->comm, s));
   }
-  NCCL_CHECK(g_nccl.GroupEnd());
-  count_launch();
+  NCCL_LAUNCH(g_nccl.GroupEnd());
   if (me == root) table_release(t);
   *out_table = to_handle(new_table(outs.release()));
   B2_CATCH

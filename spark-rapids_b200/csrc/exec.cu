@@ -344,9 +344,8 @@ struct GpuHashAggregateExec : GpuExec {
       const int64_t* count = j < nc ? t->cols[nk + na + j]->data.as<int64_t>() : nullptr;
       Column* f = new_column(B2_INT8, 0, t->rows, false);
       flags.v.push_back(f); flagged.push_back(i);
-      poisoned_sums_kernel<<<grid_for(t->rows, 256), 256, 0, stream()>>>(s->validity(), count, t->rows, f->data.as<int8_t>(), npois.as<unsigned long long>());
-      CUDA_CHECK(cudaGetLastError());
-      count_launch();
+      launch(poisoned_sums_kernel, grid_for(t->rows, 256), 256, 0, stream(), s->validity(), count, t->rows, f->data.as<int8_t>(),
+             npois.as<unsigned long long>());
     }
     unsigned long long hpois = 0;
     if (!flagged.empty()) { d2h(&hpois, npois.p, 1); sync(); }
@@ -365,10 +364,8 @@ struct GpuHashAggregateExec : GpuExec {
     TableRef r(scan_aggregate(p.get(), false, src.t, key_outs.data(), nk, m.data(), (int)m.size()));
     for (size_t q = 0; q < flagged.size(); q++) {
       Column* s = r.t->cols[nk + flagged[q]];
-      clear_poisoned_kernel<<<grid_for((r.t->rows + 31) / 32, 256), 256, 0, stream()>>>(s->valid.as<uint32_t>(), r.t->cols[nk + na + nc + q]->data.as<int8_t>(),
-                                                                                        r.t->rows);
-      CUDA_CHECK(cudaGetLastError());
-      count_launch();
+      launch(clear_poisoned_kernel, grid_for((r.t->rows + 31) / 32, 256), 256, 0, stream(), s->valid.as<uint32_t>(),
+             r.t->cols[nk + na + nc + q]->data.as<int8_t>(), r.t->rows);
       s->null_count = -1;
     }
     std::vector<Column*> out(r.t->cols.begin(), r.t->cols.begin() + nk + na + (mode == B2_AGG_MODE_PARTIAL ? nc : 0));
@@ -805,9 +802,7 @@ struct GpuOutOfCoreSortExec : GpuExec {
       }
       std::vector<Piece> pieces = with_retry([&] {
         ColGuard ord(new_column(B2_INT64, 0, in.t->rows, false));
-        ordinal_kernel<<<grid_for(in.t->rows, 256), 256, 0, stream()>>>(ord.c->data.as<int64_t>(), in.t->rows, ordinal_base);
-        CUDA_CHECK(cudaGetLastError());
-        count_launch();
+        launch(ordinal_kernel, grid_for(in.t->rows, 256), 256, 0, stream(), ord.c->data.as<int64_t>(), in.t->rows, ordinal_base);
         std::vector<Column*> cols(in.t->cols.begin(), in.t->cols.end());
         for (Column* c : cols) col_incref(c);
         cols.push_back(ord.release());

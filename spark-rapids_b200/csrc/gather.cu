@@ -97,9 +97,8 @@ static Column* gather_string(const Column* ic, const int32_t* d_map, int64_t n, 
     oc->data = DevBuf(0);
     return oc.release();
   }
-  string_sizes_kernel<<<grid_for(n, 256), 256, 0, stream()>>>(ic->offsets.as<int32_t>(), d_map, n, ic->size, ic->validity(),
-                                                              oc->offsets.as<int32_t>(), oc->valid.as<uint32_t>());
-  count_launch();
+  launch(string_sizes_kernel, grid_for(n, 256), 256, 0, stream(), ic->offsets.as<int32_t>(), d_map, n, ic->size, ic->validity(),
+         oc->offsets.as<int32_t>(), oc->valid.as<uint32_t>());
   DevBuf sums = exclusive_scan<int32_t, int32_t>(oc->offsets.as<int32_t>(), oc->offsets.as<int32_t>(), n, true);
   int64_t total = 0;
   int64_t ntiles = (n + SCAN_TILE - 1) / SCAN_TILE;
@@ -108,11 +107,9 @@ static Column* gather_string(const Column* ic, const int32_t* d_map, int64_t n, 
   if (total > 0x7fffffffLL) throw Error(B2_ERR_SIZE_OVERFLOW, "gathered string column exceeds 2^31-1 chars");
   oc->chars_bytes = total;
   oc->data = DevBuf((size_t)total);
-  if (total) {
-    string_copy_kernel<<<grid_for(n * 32, 256), 256, 0, stream()>>>(ic->offsets.as<int32_t>(), ic->data.as<uint8_t>(), d_map, n, ic->size,
-                                                                     oc->offsets.as<int32_t>(), oc->data.as<uint8_t>());
-    count_launch();
-  }
+  if (total)
+    launch(string_copy_kernel, grid_for(n * 32, 256), 256, 0, stream(), ic->offsets.as<int32_t>(), ic->data.as<uint8_t>(), d_map, n, ic->size,
+           oc->offsets.as<int32_t>(), oc->data.as<uint8_t>());
   return oc.release();
 }
 
@@ -129,10 +126,7 @@ Table* gather_table(const Table* t, const int32_t* d_map, int64_t n, bool nullif
   std::vector<int> fixed_slots;
   auto flush = [&]() {
     if (gc.ncols == 0 || n == 0) { gc.ncols = 0; return; }
-    KernelTimer kt_gather_fixed_kernel("gather_fixed_kernel");
-    gather_fixed_kernel<<<grid_for(n, 256), 256, 0, stream()>>>(gc, d_map, n, t->rows);
-    CUDA_CHECK(cudaGetLastError());
-    count_launch();
+    launch("gather_fixed_kernel", gather_fixed_kernel, grid_for(n, 256), 256, 0, stream(), gc, d_map, n, t->rows);
     gc.ncols = 0;
   };
   for (size_t k = 0; k < cols.size(); k++) {
@@ -193,9 +187,8 @@ Table* concat_tables(const std::vector<const Table*>& ts) {
       for (auto* t : ts) {
         const Column* ic = t->cols[c];
         if (ic->size) {
-          rebase_offsets_kernel<<<grid_for(ic->size, 256), 256, 0, stream()>>>(ic->offsets.as<int32_t>(), ic->size, (int32_t)ch,
-                                                                                oc->offsets.as<int32_t>() + row);
-          count_launch();
+          launch(rebase_offsets_kernel, grid_for(ic->size, 256), 256, 0, stream(), ic->offsets.as<int32_t>(), ic->size, (int32_t)ch,
+                 oc->offsets.as<int32_t>() + row);
           if (ic->chars_bytes)
             CUDA_CHECK(cudaMemcpyAsync(oc->data.as<char>() + ch, ic->data.p, (size_t)ic->chars_bytes, cudaMemcpyDeviceToDevice, stream()));
         }
@@ -224,10 +217,7 @@ Table* concat_tables(const std::vector<const Table*>& ts) {
       int64_t row = 0;
       for (auto* t : ts) {
         const Column* ic = t->cols[c];
-        if (ic->size) {
-          copy_bits_kernel<<<grid_for(ic->size, 256), 256, 0, stream()>>>(ic->validity(), 0, oc->valid.as<uint32_t>(), row, ic->size);
-          count_launch();
-        }
+        if (ic->size) launch(copy_bits_kernel, grid_for(ic->size, 256), 256, 0, stream(), ic->validity(), 0, oc->valid.as<uint32_t>(), row, ic->size);
         row += ic->size;
       }
       oc->null_count = -1;
@@ -284,20 +274,17 @@ Column* substring_column(const Column* ic, int64_t pos, int64_t len) {
   }
   if (n == 0) { CUDA_CHECK(cudaMemsetAsync(oc->offsets.p, 0, 4, stream())); oc->data = DevBuf(0); return oc.release(); }
   DevBuf starts((size_t)n * 4);
-  substring_sizes_kernel<<<grid_for(n, 256), 256, 0, stream()>>>(ic->offsets.as<int32_t>(), ic->data.as<uint8_t>(), ic->validity(), n, pos, len,
-                                                                 oc->offsets.as<int32_t>(), starts.as<int32_t>());
-  count_launch();
+  launch(substring_sizes_kernel, grid_for(n, 256), 256, 0, stream(), ic->offsets.as<int32_t>(), ic->data.as<uint8_t>(), ic->validity(), n, pos, len,
+         oc->offsets.as<int32_t>(), starts.as<int32_t>());
   DevBuf sums = exclusive_scan<int32_t, int32_t>(oc->offsets.as<int32_t>(), oc->offsets.as<int32_t>(), n, true);
   int64_t total = 0;
   d2h(&total, sums.as<int64_t>() + (n + SCAN_TILE - 1) / SCAN_TILE, 1);
   sync();
   oc->chars_bytes = total;
   oc->data = DevBuf((size_t)total);
-  if (total) {
-    substring_copy_kernel<<<grid_for(n, 256), 256, 0, stream()>>>(ic->data.as<uint8_t>(), starts.as<int32_t>(), oc->offsets.as<int32_t>(), n, oc->data.as<uint8_t>());
-    CUDA_CHECK(cudaGetLastError());
-    count_launch();
-  }
+  if (total)
+    launch(substring_copy_kernel, grid_for(n, 256), 256, 0, stream(), ic->data.as<uint8_t>(), starts.as<int32_t>(), oc->offsets.as<int32_t>(), n,
+           oc->data.as<uint8_t>());
   sync();   // `starts` is freed on return
   return oc.release();
 }
@@ -306,7 +293,7 @@ Table* slice_table(const Table* t, int64_t start, int64_t end) {
   B2_CHECK(start >= 0 && end >= start && end <= t->rows, "slice out of range");
   int64_t n = end - start;
   DevBuf map((size_t)std::max<int64_t>(n, 1) * 4);
-  if (n) { iota_kernel<<<grid_for(n, 256), 256, 0, stream()>>>(map.as<int32_t>(), n, (int32_t)start); count_launch(); }
+  if (n) launch(iota_kernel, grid_for(n, 256), 256, 0, stream(), map.as<int32_t>(), n, (int32_t)start);
   return gather_table(t, map.as<int32_t>(), n, false, nullptr);
 }
 

@@ -257,12 +257,7 @@ static Table* partition_table_direct(const Table* t, const int32_t* d_pids, int3
   const int64_t ntiles = (n + PT_TILE - 1) / PT_TILE;
   const int64_t cells = (int64_t)nparts * ntiles;
   DevBuf cnt((size_t)(cells + 1) * 4);
-  {
-    KernelTimer kt("part_tile_hist_kernel");
-    part_tile_hist_kernel<<<(int)ntiles, PT_NT, 0, stream()>>>(PidArray{d_pids}, n, nparts, ntiles, cnt.as<int32_t>());
-    CUDA_CHECK(cudaGetLastError());
-    count_launch();
-  }
+  launch("part_tile_hist_kernel", part_tile_hist_kernel<PidArray>, (int)ntiles, PT_NT, 0, stream(), PidArray{d_pids}, n, nparts, ntiles, cnt.as<int32_t>());
   DevBuf sums = exclusive_scan<int32_t, int32_t>(cnt.as<int32_t>(), cnt.as<int32_t>(), cells, true);
   std::vector<int32_t> h(nparts + 1, 0);
   CUDA_CHECK(cudaMemcpy2DAsync(h.data(), 4, cnt.p, (size_t)ntiles * 4, 4, (size_t)nparts, cudaMemcpyDeviceToHost, stream()));
@@ -282,12 +277,7 @@ static Table* partition_table_direct(const Table* t, const int32_t* d_pids, int3
   }
   DevBuf map;
   if (!via_map.empty()) map = DevBuf((size_t)n * 4);
-  {
-    KernelTimer kt("part_scatter_kernel");
-    part_scatter_kernel<<<(int)ntiles, PT_NT, 0, stream()>>>(d_pids, n, nparts, ntiles, cnt.as<int32_t>(), sc, map.as<int32_t>());
-    CUDA_CHECK(cudaGetLastError());
-    count_launch();
-  }
+  launch("part_scatter_kernel", part_scatter_kernel, (int)ntiles, PT_NT, 0, stream(), d_pids, n, nparts, ntiles, cnt.as<int32_t>(), sc, map.as<int32_t>());
   sync();
   if (h[nparts] != n) throw Error(B2_ERR_INVALID, "partition ids out of range");
   for (int p = 0; p <= nparts; p++) offsets_out[p] = h[p];
@@ -309,23 +299,11 @@ void partition_scatter_by_hash(const uint32_t* d_hash, int shift, int bits, int6
   const int64_t ntiles = (n + PT_TILE - 1) / PT_TILE;
   const int64_t cells = (int64_t)nparts * ntiles;
   DevBuf cnt((size_t)(cells + 1) * 4);
-  {
-    KernelTimer kt("part_tile_hist_kernel");
-    part_tile_hist_kernel<<<(int)ntiles, PT_NT, 0, stream()>>>(pid, n, nparts, ntiles, cnt.as<int32_t>());
-    CUDA_CHECK(cudaGetLastError());
-    count_launch();
-  }
+  launch("part_tile_hist_kernel", part_tile_hist_kernel<HashDigit>, (int)ntiles, PT_NT, 0, stream(), pid, n, nparts, ntiles, cnt.as<int32_t>());
   DevBuf sums = exclusive_scan<int32_t, int32_t>(cnt.as<int32_t>(), cnt.as<int32_t>(), cells, true);
-  {
-    int maxw = 1;
-    for (int c = 0; c < sc.n; c++) maxw = std::max(maxw, sc.width[c]);
-    const int smem = PT_TILE * maxw;
-    if (smem > 32 * 1024) CUDA_CHECK(cudaFuncSetAttribute(part_scatter2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    KernelTimer kt("part_scatter2_kernel");
-    part_scatter2_kernel<<<(int)ntiles, PT_NT, smem, stream()>>>(pid, n, nparts, ntiles, cnt.as<int32_t>(), sc);
-    CUDA_CHECK(cudaGetLastError());
-    count_launch();
-  }
+  int maxw = 1;
+  for (int c = 0; c < sc.n; c++) maxw = std::max(maxw, sc.width[c]);
+  launch("part_scatter2_kernel", part_scatter2_kernel, (int)ntiles, PT_NT, PT_TILE * maxw, stream(), pid, n, nparts, ntiles, cnt.as<int32_t>(), sc);
   sync();   // cnt / sums are freed on return
 }
 
@@ -338,16 +316,14 @@ Table* partition_table(const Table* t, const int32_t* d_pids, int32_t nparts, in
   CUDA_CHECK(cudaMemsetAsync(counts.p, 0, counts.bytes, stream()));
   std::vector<int32_t> h(nparts, 0);
   if (n) {
-    part_hist_kernel<<<grid_for(n, 256), 256, 0, stream()>>>(d_pids, n, nparts, counts.as<int32_t>());
-    count_launch();
+    launch(part_hist_kernel, grid_for(n, 256), 256, 0, stream(), d_pids, n, nparts, counts.as<int32_t>());
     d2h(h.data(), counts.p, nparts);
   }
   DevBuf ka((size_t)std::max<int64_t>(n, 1) * 8), kb((size_t)std::max<int64_t>(n, 1) * 8);
   DevBuf va((size_t)std::max<int64_t>(n, 1) * 4), vb((size_t)std::max<int64_t>(n, 1) * 4);
   int which = 0;
   if (n) {
-    pid_keys_kernel<<<grid_for(n, 256), 256, 0, stream()>>>(d_pids, n, ka.as<uint64_t>(), va.as<int32_t>());
-    count_launch();
+    launch(pid_keys_kernel, grid_for(n, 256), 256, 0, stream(), d_pids, n, ka.as<uint64_t>(), va.as<int32_t>());
     int nbytes = nparts <= 256 ? 1 : (nparts <= 65536 ? 2 : 4);
     which = radix_sort_pairs(ka.as<uint64_t>(), va.as<int32_t>(), kb.as<uint64_t>(), vb.as<int32_t>(), n, nbytes);
   }
@@ -369,11 +345,7 @@ int b2_murmur3(b2_handle table, const int32_t* cols, int32_t ncols, int32_t seed
   Table* t = table_from(table);
   KeyCols keys = key_cols_of(t, cols, ncols);
   ColGuard out(new_column(B2_INT32, 0, t->rows, false));
-  if (t->rows) {
-    murmur_kernel<<<grid_for(t->rows, 256), 256, 0, stream()>>>(keys, t->rows, (uint32_t)seed, 0, out.c->data.as<int32_t>());
-    CUDA_CHECK(cudaGetLastError());
-    count_launch();
-  }
+  if (t->rows) launch(murmur_kernel, grid_for(t->rows, 256), 256, 0, stream(), keys, t->rows, (uint32_t)seed, 0, out.c->data.as<int32_t>());
   *out_int32_col = to_handle(out.release());
   B2_CATCH
 }
@@ -385,12 +357,7 @@ int b2_hash_partition(b2_handle table, const int32_t* key_cols, int32_t nkeys, i
   B2_CHECK(num_partitions >= 1, "need at least one partition");
   KeyCols keys = key_cols_of(t, key_cols, nkeys);
   DevBuf pids((size_t)std::max<int64_t>(t->rows, 1) * 4);
-  if (t->rows) {
-    KernelTimer kt_murmur_pmod_kernel("murmur_pmod_kernel");
-    murmur_kernel<<<grid_for(t->rows, 256), 256, 0, stream()>>>(keys, t->rows, (uint32_t)seed, num_partitions, pids.as<int32_t>());
-    CUDA_CHECK(cudaGetLastError());
-    count_launch();
-  }
+  if (t->rows) launch("murmur_pmod_kernel", murmur_kernel, grid_for(t->rows, 256), 256, 0, stream(), keys, t->rows, (uint32_t)seed, num_partitions, pids.as<int32_t>());
   *out_table = to_handle(partition_table(t, pids.as<int32_t>(), num_partitions, offsets_out));
   B2_CATCH
 }

@@ -444,13 +444,10 @@ __global__ void invert_flags_kernel(int8_t* __restrict__ flags, int64_t n) {
 Column* rows_with_passing_pair(const Column* left_map, const Column* pass, int64_t stream_rows, bool invert) {
   ColGuard flags(new_column(B2_BOOL8, 0, stream_rows, false));
   if (stream_rows) CUDA_CHECK(cudaMemsetAsync(flags.c->data.p, 0, (size_t)stream_rows, stream()));
-  if (left_map->size) {
-    mark_passing_kernel<<<grid_for(left_map->size, 256), 256, 0, stream()>>>(left_map->data.as<int32_t>(), pass->data.as<int8_t>(), pass->validity(), left_map->size,
-                                                                              flags.c->data.as<int8_t>());
-    count_launch();
-  }
-  if (invert && stream_rows) { invert_flags_kernel<<<grid_for(stream_rows, 256), 256, 0, stream()>>>(flags.c->data.as<int8_t>(), stream_rows); count_launch(); }
-  CUDA_CHECK(cudaGetLastError());
+  if (left_map->size)
+    launch(mark_passing_kernel, grid_for(left_map->size, 256), 256, 0, stream(), left_map->data.as<int32_t>(), pass->data.as<int8_t>(), pass->validity(),
+           left_map->size, flags.c->data.as<int8_t>());
+  if (invert && stream_rows) launch(invert_flags_kernel, grid_for(stream_rows, 256), 256, 0, stream(), flags.c->data.as<int8_t>(), stream_rows);
   return flags.release();
 }
 
@@ -479,17 +476,14 @@ bool join_probe_pred(b2_handle ht, const Table* batch, int key_col, const Progra
   DevBuf tot(16);
   CUDA_CHECK(cudaMemsetAsync(tot.p, 0, 16, stream()));
   {
-    KernelTimer kt("join_filter_probe_kernel");
     const int grid = grid_for(n, FP_TILE, FP_CTAS);
     const uint64_t* sl = jt->slots.as<uint64_t>(); const uint32_t msk = (uint32_t)(jt->cap - 1);
     const unsigned long long* bl = jt->bloom.as<unsigned long long>();
     unsigned long long* tp = tot.as<unsigned long long>();
-    if (pw == 8) join_filter_probe_kernel<int64_t><<<grid, SF_NT, 0, stream()>>>(sp, pc->data.as<int64_t>(), n, sl, msk, bl, jt->bloom_mask, tp,
-                                                                                 lm.c->data.as<int32_t>(), rm.c->data.as<int32_t>(), tp + 1);
-    else join_filter_probe_kernel<int32_t><<<grid, SF_NT, 0, stream()>>>(sp, pc->data.as<int32_t>(), n, sl, msk, bl, jt->bloom_mask, tp,
-                                                                        lm.c->data.as<int32_t>(), rm.c->data.as<int32_t>(), tp + 1);
-    CUDA_CHECK(cudaGetLastError());
-    count_launch();
+    if (pw == 8) launch("join_filter_probe_kernel", join_filter_probe_kernel<int64_t>, grid, SF_NT, 0, stream(), sp, pc->data.as<int64_t>(), n, sl, msk, bl,
+                        jt->bloom_mask, tp, lm.c->data.as<int32_t>(), rm.c->data.as<int32_t>(), tp + 1);
+    else launch("join_filter_probe_kernel", join_filter_probe_kernel<int32_t>, grid, SF_NT, 0, stream(), sp, pc->data.as<int32_t>(), n, sl, msk, bl,
+                jt->bloom_mask, tp, lm.c->data.as<int32_t>(), rm.c->data.as<int32_t>(), tp + 1);
   }
   unsigned long long h[2] = {0, 0};
   d2h(h, tot.p, 2);
@@ -545,11 +539,8 @@ int b2_join_build(b2_handle build_keys_table, int32_t nulls_equal, b2_handle* ou
   CUDA_CHECK(cudaMemsetAsync(dups.p, 0, 4, stream()));
   if (t->rows) {
     KeyCols keys = key_cols_of(t, jt->key_idx.data(), (int)jt->key_idx.size());
-    KernelTimer kt_join_build_kernel("join_build_kernel");
-    join_build_kernel<<<grid_for(t->rows, 256), 256, 0, stream()>>>(keys, t->rows, jt->slots.as<uint64_t>(), (uint32_t)(cap - 1),
-                                                                    jt->nulls_equal, jt->fast, dups.as<int32_t>(), jt->bloom.as<unsigned long long>(), jt->bloom_mask);
-    CUDA_CHECK(cudaGetLastError());
-    count_launch();
+    launch("join_build_kernel", join_build_kernel, grid_for(t->rows, 256), 256, 0, stream(), keys, t->rows, jt->slots.as<uint64_t>(), (uint32_t)(cap - 1),
+           jt->nulls_equal, jt->fast, dups.as<int32_t>(), jt->bloom.as<unsigned long long>(), jt->bloom_mask);
   }
   int32_t h_dups = 0;
   d2h(&h_dups, dups.p, 1);
@@ -621,9 +612,8 @@ int b2_join_probe_sel(b2_handle ht, b2_handle probe_keys_table, b2_handle select
     CUDA_CHECK(cudaMemsetAsync(matched.p, 0, matched.bytes, stream()));
     int32_t extra = 0;
     if (nb) {
-      if (m) mark_matched_kernel<<<grid_for(m, 256), 256, 0, stream()>>>(ro.c->data.as<int32_t>(), m, matched.as<uint8_t>());
-      unmatched_flags_kernel<<<grid_for(nb, 256), 256, 0, stream()>>>(matched.as<uint8_t>(), nb, pos.as<int32_t>());
-      count_launch(2);
+      if (m) launch(mark_matched_kernel, grid_for(m, 256), 256, 0, stream(), ro.c->data.as<int32_t>(), m, matched.as<uint8_t>());
+      launch(unmatched_flags_kernel, grid_for(nb, 256), 256, 0, stream(), matched.as<uint8_t>(), nb, pos.as<int32_t>());
       exclusive_scan<int32_t, int32_t>(pos.as<int32_t>(), pos.as<int32_t>(), nb, true);
       d2h(&extra, pos.as<int32_t>() + nb, 1);
       sync();
@@ -634,12 +624,9 @@ int b2_join_probe_sel(b2_handle ht, b2_handle probe_keys_table, b2_handle select
       CUDA_CHECK(cudaMemcpyAsync(lm.c->data.p, lo.c->data.p, (size_t)m * 4, cudaMemcpyDeviceToDevice, stream()));
       CUDA_CHECK(cudaMemcpyAsync(rm.c->data.p, ro.c->data.p, (size_t)m * 4, cudaMemcpyDeviceToDevice, stream()));
     }
-    if (extra) {
-      append_unmatched_kernel<<<grid_for(nb, 256), 256, 0, stream()>>>(matched.as<uint8_t>(), pos.as<int32_t>(), nb, m, lm.c->data.as<int32_t>(),
-                                                                        rm.c->data.as<int32_t>());
-      CUDA_CHECK(cudaGetLastError());
-      count_launch();
-    }
+    if (extra)
+      launch(append_unmatched_kernel, grid_for(nb, 256), 256, 0, stream(), matched.as<uint8_t>(), pos.as<int32_t>(), nb, m, lm.c->data.as<int32_t>(),
+             rm.c->data.as<int32_t>());
     *out_left_map = to_handle(lm.release());
     *out_right_map = to_handle(rm.release());
     return B2_OK;
@@ -661,27 +648,20 @@ int b2_join_probe_sel(b2_handle ht, b2_handle probe_keys_table, b2_handle select
       const int pw = pc ? dtype_width(pc->dtype) : 0;
       if (kind == B2_JOIN_INNER && jt->fast && pc && !pc->nullable() && !is_float(pc->dtype) && pc->dtype != B2_STRING && (pw == 4 || pw == 8) &&
           n < 0x7fffffffLL && !getenv("B2_JOIN_NO_FAST_PROBE")) {
-        KernelTimer kt("join_probe_distinct1_kernel");
         const int grid = grid_for(n, 256);
         const uint64_t* sl = jt->slots.as<uint64_t>(); const uint32_t msk = (uint32_t)(jt->cap - 1);
         const unsigned long long* bl = jt->bloom.as<unsigned long long>(); unsigned long long* tp = tot.as<unsigned long long>();
         int32_t* lp = lm.c->data.as<int32_t>(); int32_t* rp = rm.c->data.as<int32_t>();
-        if (pw == 8) {
-          if (sel) join_probe_distinct1_kernel<int64_t, true><<<grid, 256, 0, stream()>>>(pc->data.as<int64_t>(), sel, n, sl, msk, bl, jt->bloom_mask, tp, lp, rp);
-          else join_probe_distinct1_kernel<int64_t, false><<<grid, 256, 0, stream()>>>(pc->data.as<int64_t>(), sel, n, sl, msk, bl, jt->bloom_mask, tp, lp, rp);
-        } else {
-          if (sel) join_probe_distinct1_kernel<int32_t, true><<<grid, 256, 0, stream()>>>(pc->data.as<int32_t>(), sel, n, sl, msk, bl, jt->bloom_mask, tp, lp, rp);
-          else join_probe_distinct1_kernel<int32_t, false><<<grid, 256, 0, stream()>>>(pc->data.as<int32_t>(), sel, n, sl, msk, bl, jt->bloom_mask, tp, lp, rp);
-        }
-        CUDA_CHECK(cudaGetLastError());
-        count_launch();
+        if (pw == 8)
+          launch("join_probe_distinct1_kernel", sel ? join_probe_distinct1_kernel<int64_t, true> : join_probe_distinct1_kernel<int64_t, false>, grid, 256, 0,
+                 stream(), pc->data.as<int64_t>(), sel, n, sl, msk, bl, jt->bloom_mask, tp, lp, rp);
+        else
+          launch("join_probe_distinct1_kernel", sel ? join_probe_distinct1_kernel<int32_t, true> : join_probe_distinct1_kernel<int32_t, false>, grid, 256, 0,
+                 stream(), pc->data.as<int32_t>(), sel, n, sl, msk, bl, jt->bloom_mask, tp, lp, rp);
       } else {
-      KernelTimer kt("join_probe_distinct_kernel");
-      join_probe_distinct_kernel<<<grid_for(n, 256), 256, 0, stream()>>>(pk, bk, n, jt->slots.as<uint64_t>(), (uint32_t)(jt->cap - 1),
-                                                                          jt->nulls_equal, jt->fast, kind, tot.as<unsigned long long>(),
-                                                                          lm.c->data.as<int32_t>(), rm.c->data.as<int32_t>(), jt->bloom.as<unsigned long long>(), jt->bloom_mask, sel);
-      CUDA_CHECK(cudaGetLastError());
-      count_launch();
+        launch("join_probe_distinct_kernel", join_probe_distinct_kernel, grid_for(n, 256), 256, 0, stream(), pk, bk, n, jt->slots.as<uint64_t>(),
+               (uint32_t)(jt->cap - 1), jt->nulls_equal, jt->fast, kind, tot.as<unsigned long long>(), lm.c->data.as<int32_t>(), rm.c->data.as<int32_t>(),
+               jt->bloom.as<unsigned long long>(), jt->bloom_mask, sel);
       }
       if (kind == B2_JOIN_INNER) { unsigned long long h = 0; d2h(&h, tot.p, 1); sync(); matched = (int64_t)h; }
     }
@@ -693,11 +673,8 @@ int b2_join_probe_sel(b2_handle ht, b2_handle probe_keys_table, b2_handle select
   DevBuf counts((size_t)std::max<int64_t>(n, 1) * 4), offsets((size_t)(n + 1) * 8);
   int64_t total = 0;
   if (n) {
-    KernelTimer kt_join_probe_count_kernel("join_probe_count_kernel");
-    join_probe_kernel<0><<<grid_for(n, 256), 256, 0, stream()>>>(pk, bk, n, jt->slots.as<uint64_t>(), (uint32_t)(jt->cap - 1), jt->nulls_equal, jt->fast, kind,
-                                                                  counts.as<int32_t>(), nullptr, nullptr, nullptr, jt->bloom.as<unsigned long long>(), jt->bloom_mask, sel);
-    CUDA_CHECK(cudaGetLastError());
-    count_launch();
+    launch("join_probe_count_kernel", join_probe_kernel<0>, grid_for(n, 256), 256, 0, stream(), pk, bk, n, jt->slots.as<uint64_t>(), (uint32_t)(jt->cap - 1),
+           jt->nulls_equal, jt->fast, kind, counts.as<int32_t>(), nullptr, nullptr, nullptr, jt->bloom.as<unsigned long long>(), jt->bloom_mask, sel);
     exclusive_scan<int32_t, int64_t>(counts.as<int32_t>(), offsets.as<int64_t>(), n, true);
     d2h(&total, offsets.as<int64_t>() + n, 1);
     sync();
@@ -707,14 +684,10 @@ int b2_join_probe_sel(b2_handle ht, b2_handle probe_keys_table, b2_handle select
   if (total > 0x7fffffffLL) throw Error(B2_ERR_SIZE_OVERFLOW, "join output exceeds 2^31-1 rows; split the stream batch");
   ColGuard lm(new_column(B2_INT32, 0, total, false));
   ColGuard rm(semi_like ? nullptr : new_column(B2_INT32, 0, total, false));
-  if (n && total) {
-    KernelTimer kt_join_probe_write_kernel("join_probe_write_kernel");
-    join_probe_kernel<1><<<grid_for(n, 256), 256, 0, stream()>>>(pk, bk, n, jt->slots.as<uint64_t>(), (uint32_t)(jt->cap - 1), jt->nulls_equal, jt->fast, kind,
-                                                                  nullptr, offsets.as<int64_t>(), lm.c->data.as<int32_t>(),
-                                                                  semi_like ? nullptr : rm.c->data.as<int32_t>(), jt->bloom.as<unsigned long long>(), jt->bloom_mask, sel);
-    CUDA_CHECK(cudaGetLastError());
-    count_launch();
-  }
+  if (n && total)
+    launch("join_probe_write_kernel", join_probe_kernel<1>, grid_for(n, 256), 256, 0, stream(), pk, bk, n, jt->slots.as<uint64_t>(), (uint32_t)(jt->cap - 1),
+           jt->nulls_equal, jt->fast, kind, nullptr, offsets.as<int64_t>(), lm.c->data.as<int32_t>(), semi_like ? nullptr : rm.c->data.as<int32_t>(),
+           jt->bloom.as<unsigned long long>(), jt->bloom_mask, sel);
   *out_left_map = to_handle(lm.release());
   if (out_right_map) *out_right_map = semi_like ? 0 : to_handle(rm.release());
   B2_CATCH

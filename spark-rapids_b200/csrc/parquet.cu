@@ -1367,20 +1367,12 @@ Table* parquet_decode(const uint8_t* host, const uint8_t* dev_in, int64_t len, c
       CUDA_CHECK(cudaEventRecord(ev_fork, s));
       CUDA_CHECK(cudaStreamWaitEvent(ws, ev_fork, 0));
     }
-    {
-      KernelTimer kt("snappy_big_kernel");
-      snappy_big_kernel<<<(int)todo_big.size(), SB_WARPS * 32, 0, s>>>(d_pages.as<PageD>(), d_todo_b.as<int32_t>(), d_big_soff.as<int64_t>(), d_file,
-                                                                        scratch.as<uint8_t>(), d_big_S.as<uint32_t>(), d_big_fail.as<int32_t>());
-      CUDA_CHECK(cudaGetLastError());
-      count_launch();
-    }
+    launch("snappy_big_kernel", snappy_big_kernel, (int)todo_big.size(), SB_WARPS * 32, 0, s, d_pages.as<PageD>(), d_todo_b.as<int32_t>(),
+           d_big_soff.as<int64_t>(), d_file, scratch.as<uint8_t>(), d_big_S.as<uint32_t>(), d_big_fail.as<int32_t>());
   }
   if (!todo_snappy.empty()) {
-    KernelTimer kt_snappy_kernel("snappy_kernel", ws);
-    snappy_kernel<<<((int)todo_snappy.size() + SN_WARPS - 1) / SN_WARPS, SN_WARPS * 32, 0, ws>>>(d_pages.as<PageD>(), d_todo_s.as<int32_t>(), (int)todo_snappy.size(), d_file,
-                                                                               scratch.as<uint8_t>(), d_err.as<int32_t>(), nullptr);
-    CUDA_CHECK(cudaGetLastError());
-    count_launch();
+    launch("snappy_kernel", snappy_kernel, ((int)todo_snappy.size() + SN_WARPS - 1) / SN_WARPS, SN_WARPS * 32, 0, ws, d_pages.as<PageD>(),
+           d_todo_s.as<int32_t>(), (int)todo_snappy.size(), d_file, scratch.as<uint8_t>(), d_err.as<int32_t>(), nullptr);
     if (ev_join) CUDA_CHECK(cudaEventRecord(ev_join, ws));
   }
   if (!todo_big.empty()) {
@@ -1388,18 +1380,11 @@ Table* parquet_decode(const uint8_t* host, const uint8_t* dev_in, int64_t len, c
       KernelTimer kt("snappy_jump_resolve_kernels");
       const uint32_t total = (uint32_t)big_S;
       const int grid = grid_for((int64_t)total, 256 * 4, 8);
-      for (int round = 0; round < 20; round++) snappy_jump_kernel<<<grid, 256, 0, s>>>(d_big_S.as<uint32_t>(), total);
-      snappy_resolve_kernel<<<grid_for((int64_t)total, 256, 8), 256, 0, s>>>(d_big_S.as<uint32_t>(), scratch.as<uint8_t>() + big_region, total);
-      CUDA_CHECK(cudaGetLastError());
-      count_launch(21);
+      for (int round = 0; round < 20; round++) launch(snappy_jump_kernel, grid, 256, 0, s, d_big_S.as<uint32_t>(), total);
+      launch(snappy_resolve_kernel, grid_for((int64_t)total, 256, 8), 256, 0, s, d_big_S.as<uint32_t>(), scratch.as<uint8_t>() + big_region, total);
     }
-    {
-      KernelTimer kt_fb("snappy_fallback_kernel");
-      snappy_kernel<<<((int)todo_big.size() + SN_WARPS - 1) / SN_WARPS, SN_WARPS * 32, 0, s>>>(d_pages.as<PageD>(), d_todo_b.as<int32_t>(), (int)todo_big.size(), d_file,
-                                                                                               scratch.as<uint8_t>(), d_err.as<int32_t>(), d_big_fail.as<int32_t>());
-      CUDA_CHECK(cudaGetLastError());
-      count_launch();
-    }
+    launch("snappy_fallback_kernel", snappy_kernel, ((int)todo_big.size() + SN_WARPS - 1) / SN_WARPS, SN_WARPS * 32, 0, s, d_pages.as<PageD>(),
+           d_todo_b.as<int32_t>(), (int)todo_big.size(), d_file, scratch.as<uint8_t>(), d_err.as<int32_t>(), d_big_fail.as<int32_t>());
   }
   if (ev_join) {
     CUDA_CHECK(cudaStreamWaitEvent(s, ev_join, 0));
@@ -1408,11 +1393,8 @@ Table* parquet_decode(const uint8_t* host, const uint8_t* dev_in, int64_t len, c
   std::vector<int64_t> col_nonnull(ncols, 0);
   std::vector<bool> has_nulls(ncols, false);
   if (!todo_levels.empty()) {
-    KernelTimer kt_levels_kernel("levels_kernel");
-    levels_kernel<<<(int)todo_levels.size(), PQ_NT, 0, s>>>(d_pages.as<PageD>(), d_todo_l.as<int32_t>(), d_chunks.as<ChunkD>(), d_cols.as<ColD>(), d_file,
-                                                            scratch.as<uint8_t>(), d_nonnull.as<int32_t>());
-    CUDA_CHECK(cudaGetLastError());
-    count_launch();
+    launch("levels_kernel", levels_kernel, (int)todo_levels.size(), PQ_NT, 0, s, d_pages.as<PageD>(), d_todo_l.as<int32_t>(), d_chunks.as<ChunkD>(),
+           d_cols.as<ColD>(), d_file, scratch.as<uint8_t>(), d_nonnull.as<int32_t>());
     std::vector<int32_t> nn(pages.size());
     d2h(nn.data(), d_nonnull.p, nn.size());
     sync();
@@ -1431,26 +1413,18 @@ Table* parquet_decode(const uint8_t* host, const uint8_t* dev_in, int64_t len, c
       for (int c = 0; c < ncols; c++) hn[c] = has_nulls[c] ? 1 : 0;
       DevBuf d_hn((size_t)ncols);
       h2d(d_hn.p, hn.data(), hn.size());
-      fill_uniform_levels_kernel<<<(int)todo_levels.size(), PQ_NT, 0, s>>>(d_pages.as<PageD>(), d_todo_l.as<int32_t>(), d_chunks.as<ChunkD>(), d_cols.as<ColD>(),
-                                                                           d_nonnull.as<int32_t>(), d_hn.as<uint8_t>());
-      CUDA_CHECK(cudaGetLastError());
-      count_launch();
+      launch(fill_uniform_levels_kernel, (int)todo_levels.size(), PQ_NT, 0, s, d_pages.as<PageD>(), d_todo_l.as<int32_t>(), d_chunks.as<ChunkD>(),
+             d_cols.as<ColD>(), d_nonnull.as<int32_t>(), d_hn.as<uint8_t>());
     }
   }
   DevBuf d_dict_src((size_t)std::max<int64_t>(dict_str_total, 1) * 8), d_dict_len((size_t)std::max<int64_t>(dict_str_total, 1) * 4);
-  if (dict_str_total) {
-    dict_strings_kernel<<<((int)chunks.size() + 63) / 64, 64, 0, s>>>(d_pages.as<PageD>(), d_chunks.as<ChunkD>(), (int)chunks.size(), d_file,
-                                                                       scratch.as<uint8_t>(), d_dict_src.as<int64_t>(), d_dict_len.as<int32_t>(), d_err.as<int32_t>());
-    count_launch();
-  }
-  if (!todo_values.empty()) {
-    KernelTimer kt_values_kernel("values_kernel");
-    values_kernel<<<(int)todo_values.size(), PQ_NT, 0, s>>>(d_pages.as<PageD>(), d_todo_v.as<int32_t>(), d_chunks.as<ChunkD>(), d_cols.as<ColD>(), d_file,
-                                                            scratch.as<uint8_t>(), d_nonnull.as<int32_t>(), d_dict_src.as<int64_t>(), d_dict_len.as<int32_t>(),
-                                                            d_err.as<int32_t>());
-    CUDA_CHECK(cudaGetLastError());
-    count_launch();
-  }
+  if (dict_str_total)
+    launch(dict_strings_kernel, ((int)chunks.size() + 63) / 64, 64, 0, s, d_pages.as<PageD>(), d_chunks.as<ChunkD>(), (int)chunks.size(), d_file,
+           scratch.as<uint8_t>(), d_dict_src.as<int64_t>(), d_dict_len.as<int32_t>(), d_err.as<int32_t>());
+  if (!todo_values.empty())
+    launch("values_kernel", values_kernel, (int)todo_values.size(), PQ_NT, 0, s, d_pages.as<PageD>(), d_todo_v.as<int32_t>(), d_chunks.as<ChunkD>(),
+           d_cols.as<ColD>(), d_file, scratch.as<uint8_t>(), d_nonnull.as<int32_t>(), d_dict_src.as<int64_t>(), d_dict_len.as<int32_t>(),
+           d_err.as<int32_t>());
   // assemble output columns
   ColsGuard outs;
   for (int c = 0; c < ncols; c++) {
@@ -1468,11 +1442,9 @@ Table* parquet_decode(const uint8_t* host, const uint8_t* dev_in, int64_t len, c
       DevBuf xl, xs;
       if (has_nulls[c]) {
         xl = DevBuf((size_t)(total_rows + 1) * 4); xs = DevBuf((size_t)std::max<int64_t>(total_rows, 1) * 8);
-        if (total_rows) {
-          expand_null_lengths_kernel<<<grid_for(total_rows, 256), 256, 0, s>>>(lvl[c].as<uint8_t>(), idx.as<int64_t>(), total_rows, lens, srcs, xl.as<int32_t>(),
-                                                                                xs.as<int64_t>(), oc->valid.as<uint32_t>());
-          count_launch();
-        }
+        if (total_rows)
+          launch(expand_null_lengths_kernel, grid_for(total_rows, 256), 256, 0, s, lvl[c].as<uint8_t>(), idx.as<int64_t>(), total_rows, lens, srcs,
+                 xl.as<int32_t>(), xs.as<int64_t>(), oc->valid.as<uint32_t>());
         lens = xl.as<int32_t>(); srcs = xs.as<int64_t>();
       }
       oc->offsets = DevBuf((size_t)(total_rows + 1) * 4);
@@ -1484,15 +1456,13 @@ Table* parquet_decode(const uint8_t* host, const uint8_t* dev_in, int64_t len, c
       oc->chars_bytes = chars;
       oc->data = DevBuf((size_t)chars);
       if (chars) {
-        string_chars_kernel<<<grid_for(total_rows * 32, 256), 256, 0, s>>>(srcs, oc->offsets.as<int32_t>(), total_rows, oc->data.as<uint8_t>());
-        count_launch();
+        launch(string_chars_kernel, grid_for(total_rows * 32, 256), 256, 0, s, srcs, oc->offsets.as<int32_t>(), total_rows, oc->data.as<uint8_t>());
         sync();  // srcs / scratch are read by the kernel; keep them alive
       }
     } else if (has_nulls[c]) {
       oc->data = DevBuf((size_t)total_rows * plans[c].out_width);
-      expand_nulls_kernel<<<grid_for(total_rows, 256), 256, 0, s>>>(lvl[c].as<uint8_t>(), idx.as<int64_t>(), total_rows, plans[c].out_width,
-                                                                     dense[c].as<uint8_t>(), oc->data.as<uint8_t>(), oc->valid.as<uint32_t>());
-      count_launch();
+      launch(expand_nulls_kernel, grid_for(total_rows, 256), 256, 0, s, lvl[c].as<uint8_t>(), idx.as<int64_t>(), total_rows, plans[c].out_width,
+             dense[c].as<uint8_t>(), oc->data.as<uint8_t>(), oc->valid.as<uint32_t>());
     } else {
       oc->data = std::move(dense[c]);  // no NULLs: the dense decode IS the column
     }

@@ -112,11 +112,9 @@ inline DevBuf exclusive_scan(const TIn* in, TOut* out, int64_t n, bool write_tot
     if (write_total) CUDA_CHECK(cudaMemsetAsync(out, 0, sizeof(TOut), stream()));
     return sums;
   }
-  scan_reduce_kernel<TIn><<<(int)ntiles, SCAN_NT, 0, stream()>>>(in, n, sums.as<int64_t>());
-  scan_tiles_kernel<<<1, 1024, 0, stream()>>>(sums.as<int64_t>(), ntiles);
-  scan_final_kernel<TIn, TOut><<<(int)ntiles, SCAN_NT, 0, stream()>>>(in, out, n, sums.as<int64_t>(), write_total);
-  CUDA_CHECK(cudaGetLastError());
-  count_launch(3);
+  launch(scan_reduce_kernel<TIn>, (int)ntiles, SCAN_NT, 0, stream(), in, n, sums.as<int64_t>());
+  launch(scan_tiles_kernel, 1, 1024, 0, stream(), sums.as<int64_t>(), ntiles);
+  launch(scan_final_kernel<TIn, TOut>, (int)ntiles, SCAN_NT, 0, stream(), in, out, n, sums.as<int64_t>(), write_total);
   return sums;
 }
 #endif

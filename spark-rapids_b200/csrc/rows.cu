@@ -147,11 +147,7 @@ int b2_table_to_rows(b2_handle table, uint8_t* host_rows, int64_t capacity_bytes
   for (size_t c = 0; c < t->cols.size(); c++) { L.data[c] = t->cols[c]->data.p; L.valid[c] = t->cols[c]->valid.as<uint32_t>(); }
   DevBuf rows((size_t)total);
   const int rpt = pick_rows_per_tile(L.row_bytes);
-  const int smem = rpt * L.row_bytes;
-  CUDA_CHECK(cudaFuncSetAttribute(to_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  to_rows_kernel<<<grid_for(t->rows, rpt, 2), 256, smem, stream()>>>(L, t->rows, rpt, rows.as<uint8_t>());
-  CUDA_CHECK(cudaGetLastError());
-  count_launch();
+  launch(to_rows_kernel, grid_for(t->rows, rpt, 2), 256, rpt * L.row_bytes, stream(), L, t->rows, rpt, rows.as<uint8_t>());
   CUDA_CHECK(cudaMemcpyAsync(host_rows, rows.p, (size_t)total, cudaMemcpyDeviceToHost, stream()));
   sync();
   B2_CATCH
@@ -171,11 +167,7 @@ int b2_table_from_rows(const uint8_t* host_rows, int64_t nrows, const int32_t* d
     DevBuf rows((size_t)total);
     CUDA_CHECK(cudaMemcpyAsync(rows.p, host_rows, (size_t)total, cudaMemcpyHostToDevice, stream()));
     const int rpt = pick_rows_per_tile(L.row_bytes);
-    const int smem = rpt * L.row_bytes;
-    CUDA_CHECK(cudaFuncSetAttribute(from_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    from_rows_kernel<<<grid_for(nrows, rpt, 2), 256, smem, stream()>>>(L, nrows, rpt, rows.as<uint8_t>());
-    CUDA_CHECK(cudaGetLastError());
-    count_launch();
+    launch(from_rows_kernel, grid_for(nrows, rpt, 2), 256, rpt * L.row_bytes, stream(), L, nrows, rpt, rows.as<uint8_t>());
     sync();
   }
   *out_table = to_handle(new_table(outs.release()));

@@ -345,12 +345,6 @@ void fill_inputs(VMInputs& in, const Table* t) {
   for (int i = 0; i < n; i++) { in.data[i] = t->cols[i]->data.p; in.valid[i] = t->cols[i]->validity(); in.offsets[i] = t->cols[i]->offsets.as<int32_t>(); }
 }
 
-template <typename K>
-static void set_dyn_smem(K kernel, int bytes) {
-  // static (program image, ~10 KB) + dynamic must stay under 48 KB unless the kernel opts in
-  if (bytes > 32 * 1024) CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
-}
-
 int vm_grid(int64_t nrows, int smem_bytes, int tile_rows) {
   int64_t ntiles = (nrows + tile_rows - 1) / tile_rows;
   int per_sm = 8;  // 2048 threads / 256
@@ -416,25 +410,17 @@ static int64_t run_filter(const Program* prog, const VMInputs& in, FilterCols& f
   if (staged) {
     const int regs_bytes = (prog->hdr.bytes_per_row * st.tile_rows + 127) & ~127;
     smem = regs_bytes + st.buf_bytes;
-    CUDA_CHECK(cudaFuncSetAttribute(filter_staged_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     const int per_sm = std::max(1, std::min(4, (224 * 1024) / (smem + (int)sizeof(VMShared) + 2048)));
     grid = (int)std::max<int64_t>(1, std::min<int64_t>(ntiles, (int64_t)sm_count() * per_sm));
-    KernelTimer kt("filter_staged_kernel");
-    filter_staged_kernel<<<grid, VM_NT, smem, stream()>>>(prog->d_hdr.as<VMProgramHeader>(), prog->d_code.as<VMInstr>(), in, fc, st, fs, nrows,
-                                                          status.as<uint64_t>(), work.as<FilterWork>());
+    launch("filter_staged_kernel", filter_staged_kernel, grid, VM_NT, smem, stream(), prog->d_hdr.as<VMProgramHeader>(), prog->d_code.as<VMInstr>(), in, fc,
+           st, fs, nrows, status.as<uint64_t>(), work.as<FilterWork>());
   } else if (count_only) {
-    set_dyn_smem(filter_kernel<true>, smem);
-    KernelTimer kt_filter_count_kernel("filter_count_kernel");
-    filter_kernel<true><<<grid, VM_NT, smem, stream()>>>(prog->d_hdr.as<VMProgramHeader>(), prog->d_code.as<VMInstr>(), in, fc,
-                                                          nrows, nullptr, work.as<FilterWork>());
+    launch("filter_count_kernel", filter_kernel<true>, grid, VM_NT, smem, stream(), prog->d_hdr.as<VMProgramHeader>(), prog->d_code.as<VMInstr>(), in, fc,
+           nrows, nullptr, work.as<FilterWork>());
   } else {
-    set_dyn_smem(filter_kernel<false>, smem);
-    KernelTimer kt_filter_kernel("filter_kernel");
-    filter_kernel<false><<<grid, VM_NT, smem, stream()>>>(prog->d_hdr.as<VMProgramHeader>(), prog->d_code.as<VMInstr>(), in, fc,
-                                                           nrows, status.as<uint64_t>(), work.as<FilterWork>());
+    launch("filter_kernel", filter_kernel<false>, grid, VM_NT, smem, stream(), prog->d_hdr.as<VMProgramHeader>(), prog->d_code.as<VMInstr>(), in, fc,
+           nrows, status.as<uint64_t>(), work.as<FilterWork>());
   }
-  CUDA_CHECK(cudaGetLastError());
-  count_launch();
   FilterWork hw;
   d2h(&hw, work.p, 1);
   sync();
@@ -580,12 +566,9 @@ int b2_project(b2_handle program, b2_handle table, b2_handle* out_table) {
     computed++;
   }
   if (n > 0 && computed > 0) {
-    int smem = prog->hdr.smem_bytes;
-    set_dyn_smem(project_kernel, smem);
-    KernelTimer kt_project_kernel("project_kernel");
-    project_kernel<<<vm_grid(n, smem, prog->hdr.tile_rows), VM_NT, smem, stream()>>>(prog->d_hdr.as<VMProgramHeader>(), prog->d_code.as<VMInstr>(), in, oc, n);
-    CUDA_CHECK(cudaGetLastError());
-    count_launch();
+    const int smem = prog->hdr.smem_bytes;
+    launch("project_kernel", project_kernel, vm_grid(n, smem, prog->hdr.tile_rows), VM_NT, smem, stream(), prog->d_hdr.as<VMProgramHeader>(),
+           prog->d_code.as<VMInstr>(), in, oc, n);
   }
   *out_table = to_handle(new_table(outs.release()));
   B2_CATCH

@@ -142,13 +142,9 @@ bool simple_filter_row_ids(const Program* prog, const Table* t, Column** out) {
   DevBuf work(sizeof(SimpleWork)), status((size_t)ntiles * 8);
   CUDA_CHECK(cudaMemsetAsync(work.p, 0, sizeof(SimpleWork), stream()));
   CUDA_CHECK(cudaMemsetAsync(status.p, 0, (size_t)ntiles * 8, stream()));
-  {
-    KernelTimer kt("simple_filter_ids_kernel");
-    const int grid = (int)std::min<int64_t>(ntiles, (int64_t)sm_count() * 5);
-    simple_filter_ids_kernel<<<grid, SF_NT, 0, stream()>>>(sp, n, ids.c->data.as<int32_t>(), status.as<uint64_t>(), work.as<SimpleWork>());
-    CUDA_CHECK(cudaGetLastError());
-    count_launch();
-  }
+  const int grid = (int)std::min<int64_t>(ntiles, (int64_t)sm_count() * 5);
+  launch("simple_filter_ids_kernel", simple_filter_ids_kernel, grid, SF_NT, 0, stream(), sp, n, ids.c->data.as<int32_t>(), status.as<uint64_t>(),
+         work.as<SimpleWork>());
   SimpleWork hw;
   d2h(&hw, work.p, 1);
   sync();

@@ -111,8 +111,7 @@ int radix_sort_pairs(uint64_t* keys_a, int32_t* vals_a, uint64_t* keys_b, int32_
   if (n <= 1) return 0;
   DevBuf hist(8 * 256 * 8);
   CUDA_CHECK(cudaMemsetAsync(hist.p, 0, hist.bytes, stream()));
-  hist8_kernel<<<grid_for(n, 256 * 8), 256, 0, stream()>>>(keys_a, n, nbytes, hist.as<unsigned long long>());
-  count_launch();
+  launch(hist8_kernel, grid_for(n, 256 * 8), 256, 0, stream(), keys_a, n, nbytes, hist.as<unsigned long long>());
   std::vector<unsigned long long> h(8 * 256);
   d2h(h.data(), hist.p, h.size());
   sync();
@@ -126,14 +125,9 @@ int radix_sort_pairs(uint64_t* keys_a, int32_t* vals_a, uint64_t* keys_b, int32_
     if (trivial) continue;
     uint64_t* kin = cur ? keys_b : keys_a; int32_t* vin = cur ? vals_b : vals_a;
     uint64_t* kout = cur ? keys_a : keys_b; int32_t* vout = cur ? vals_a : vals_b;
-    KernelTimer kt_radix_tile_hist_kernel("radix_tile_hist_kernel");
-    tile_hist_kernel<<<(int)ntiles, RS_NT, 0, stream()>>>(kin, n, 8 * d, th.as<int32_t>(), ntiles);
-    count_launch();
+    launch("radix_tile_hist_kernel", tile_hist_kernel, (int)ntiles, RS_NT, 0, stream(), kin, n, 8 * d, th.as<int32_t>(), ntiles);
     exclusive_scan<int32_t, int64_t>(th.as<int32_t>(), to.as<int64_t>(), 256 * ntiles, false);
-    KernelTimer kt_radix_scatter_kernel("radix_scatter_kernel");
-    scatter_kernel<<<(int)ntiles, RS_NT, 0, stream()>>>(kin, vin, kout, vout, n, 8 * d, to.as<int64_t>(), ntiles);
-    CUDA_CHECK(cudaGetLastError());
-    count_launch();
+    launch("radix_scatter_kernel", scatter_kernel, (int)ntiles, RS_NT, 0, stream(), kin, vin, kout, vout, n, 8 * d, to.as<int64_t>(), ntiles);
     cur ^= 1;
   }
   return cur;
@@ -253,7 +247,7 @@ SortPlan make_sort_plan(const Table* t, const b2_order_by_arg* keys, int nkeys, 
     } else if (col->dtype == B2_STRING) {
       DevBuf m(4);
       CUDA_CHECK(cudaMemsetAsync(m.p, 0, 4, stream()));
-      if (col->size) { max_strlen_kernel<<<grid_for(col->size, 256), 256, 0, stream()>>>(col->offsets.as<int32_t>(), col->size, m.as<int32_t>()); count_launch(); }
+      if (col->size) launch(max_strlen_kernel, grid_for(col->size, 256), 256, 0, stream(), col->offsets.as<int32_t>(), col->size, m.as<int32_t>());
       int32_t mx = 0;
       d2h(&mx, m.p, 1);
       sync();
@@ -305,24 +299,17 @@ DevBuf sort_order(const Table* t, const b2_order_by_arg* keys, int nkeys) {
   SortPlan plan = make_sort_plan(t, keys, nkeys);
   DevBuf perm_a((size_t)std::max<int64_t>(n, 1) * 4), perm_b((size_t)std::max<int64_t>(n, 1) * 4);
   if (n == 0) return perm_a;
-  iota32_kernel<<<grid_for(n, 256), 256, 0, stream()>>>(perm_a.as<int32_t>(), n);
-  count_launch();
+  launch(iota32_kernel, grid_for(n, 256), 256, 0, stream(), perm_a.as<int32_t>(), n);
   if (n == 1) return perm_a;
   const int nchunks = (plan.key_bytes + 7) / 8;
   if (n <= SS_MAX && !getenv("B2_SORT_NO_SMALL")) {
     DevBuf kk((size_t)nchunks * n * 8);
-    for (int chunk = 0; chunk < nchunks; chunk++) {
-      build_chunk_kernel<<<grid_for(n, 256), 256, 0, stream()>>>(plan, nullptr, n, chunk, kk.as<uint64_t>() + (size_t)chunk * n);
-      count_launch();
-    }
+    for (int chunk = 0; chunk < nchunks; chunk++)
+      launch(build_chunk_kernel, grid_for(n, 256), 256, 0, stream(), plan, nullptr, n, chunk, kk.as<uint64_t>() + (size_t)chunk * n);
     int npow2 = 2;
     while (npow2 < n) npow2 <<= 1;
     const int smem = npow2 * 4;
-    if (smem > 48 * 1024) CUDA_CHECK(cudaFuncSetAttribute(small_sort_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    KernelTimer kt("small_sort_kernel");
-    small_sort_kernel<<<1, SS_NT, smem, stream()>>>(kk.as<uint64_t>(), nchunks, (int)n, npow2, perm_a.as<int32_t>());
-    CUDA_CHECK(cudaGetLastError());
-    count_launch();
+    launch("small_sort_kernel", small_sort_kernel, 1, SS_NT, smem, stream(), kk.as<uint64_t>(), nchunks, (int)n, npow2, perm_a.as<int32_t>());
     return perm_a;
   }
   DevBuf keys_a((size_t)n * 8), keys_b((size_t)n * 8);
@@ -330,9 +317,7 @@ DevBuf sort_order(const Table* t, const b2_order_by_arg* keys, int nkeys) {
   for (int chunk = nchunks - 1; chunk >= 0; chunk--) {
     int32_t* pin = in_a ? perm_a.as<int32_t>() : perm_b.as<int32_t>();
     int32_t* pout = in_a ? perm_b.as<int32_t>() : perm_a.as<int32_t>();
-    build_chunk_kernel<<<grid_for(n, 256), 256, 0, stream()>>>(plan, pin, n, chunk, keys_a.as<uint64_t>());
-    CUDA_CHECK(cudaGetLastError());
-    count_launch();
+    launch(build_chunk_kernel, grid_for(n, 256), 256, 0, stream(), plan, pin, n, chunk, keys_a.as<uint64_t>());
     // the low (8 - used) bytes of the last chunk are zero and get skipped as trivial digits
     int r = radix_sort_pairs(keys_a.as<uint64_t>(), pin, keys_b.as<uint64_t>(), pout, n, 8);
     if (r == 1) in_a = !in_a;
@@ -388,9 +373,7 @@ int64_t lower_bound_row(const Table* sorted, const Table* probe, const b2_order_
   B2_CHECK(probe->rows >= 1, "bounds: empty probe");
   std::vector<SortPlan> p = shared_sort_plans({sorted, probe}, keys, nkeys);
   DevBuf out(4);
-  bounds_kernel<<<1, 32, 0, stream()>>>(p[0], p[1], sorted->rows, 1, 0, out.as<int32_t>());
-  CUDA_CHECK(cudaGetLastError());
-  count_launch();
+  launch(bounds_kernel, 1, 32, 0, stream(), p[0], p[1], sorted->rows, 1, 0, out.as<int32_t>());
   int32_t h = 0;
   d2h(&h, out.p, 1);
   sync();
@@ -511,7 +494,7 @@ DevBuf merge_runs(const Table* t, const std::vector<int64_t>& off, const b2_orde
   B2_CHECK(!off.empty() && off.front() == 0 && off.back() == n, "merge: run offsets do not cover the table");
   if (n > 0x7fffffffLL) throw Error(B2_ERR_SIZE_OVERFLOW, "merge of more than 2^31-1 rows");
   DevBuf rows_a((size_t)std::max<int64_t>(n, 1) * 4);
-  if (n) { iota32_kernel<<<grid_for(n, 256), 256, 0, stream()>>>(rows_a.as<int32_t>(), n); count_launch(); }
+  if (n) launch(iota32_kernel, grid_for(n, 256), 256, 0, stream(), rows_a.as<int32_t>(), n);
   std::vector<int64_t> runs;   // boundaries of the non-empty runs
   for (size_t r = 0; r + 1 < off.size(); r++) {
     B2_CHECK(off[r + 1] >= off[r], "merge: run offsets decrease");
@@ -522,9 +505,7 @@ DevBuf merge_runs(const Table* t, const std::vector<int64_t>& off, const b2_orde
   if (runs.size() <= 2) return rows_a;
   const int nchunks = (plan.key_bytes + 7) / 8;
   DevBuf keys_a((size_t)n * 8), keys_b((size_t)n * 8), rows_b((size_t)n * 4);
-  build_chunk_kernel<<<grid_for(n, 256), 256, 0, stream()>>>(plan, nullptr, n, 0, keys_a.as<uint64_t>());
-  CUDA_CHECK(cudaGetLastError());
-  count_launch();
+  launch(build_chunk_kernel, grid_for(n, 256), 256, 0, stream(), plan, nullptr, n, 0, keys_a.as<uint64_t>());
   DevBuf split((size_t)((n + MP_TILE - 1) / MP_TILE + 2) * 8);
   while (runs.size() > 2) {
     const bool last = runs.size() == 3;
@@ -540,17 +521,9 @@ DevBuf merge_runs(const Table* t, const std::vector<int64_t>& off, const b2_orde
       MergeRuns m{keys_a.as<uint64_t>(), rows_a.as<int32_t>(), runs[r], runs[r + 1] - runs[r], runs[r + 2] - runs[r + 1],
                   last ? nullptr : keys_b.as<uint64_t>(), rows_b.as<int32_t>()};
       const int64_t ntiles = (m.na + m.nb + MP_TILE - 1) / MP_TILE;
-      {
-        KernelTimer kt("merge_path_partition_kernel");
-        merge_path_partition_kernel<<<(int)((ntiles + 1 + 127) / 128), 128, 0, stream()>>>(plan, nchunks, tie, m, ntiles, split.as<int64_t>());
-        CUDA_CHECK(cudaGetLastError());
-      }
-      {
-        KernelTimer kt("merge_path_kernel");
-        merge_path_kernel<<<(int)ntiles, MP_NT, 0, stream()>>>(plan, nchunks, tie, m, split.as<int64_t>());
-        CUDA_CHECK(cudaGetLastError());
-      }
-      count_launch(2);
+      launch("merge_path_partition_kernel", merge_path_partition_kernel, (int)((ntiles + 1 + 127) / 128), 128, 0, stream(), plan, nchunks, tie, m,
+             ntiles, split.as<int64_t>());
+      launch("merge_path_kernel", merge_path_kernel, (int)ntiles, MP_NT, 0, stream(), plan, nchunks, tie, m, split.as<int64_t>());
     }
     next.push_back(n);
     runs.swap(next);
@@ -594,11 +567,9 @@ static Table* top_n_select(const Table* t, const b2_order_by_arg* keys, int nkey
   // leading 8-byte chunks of the row key on which ALL rows agree cannot discriminate (e.g. the high half of a DECIMAL128
   // revenue): the selection moves on to the next chunk, every row still being a candidate
   for (int chunk = 0; chunk < nchunks && m < 0; chunk++) {
-    build_chunk_kernel<<<grid_for(n, 256), 256, 0, stream()>>>(plan, nullptr, n, chunk, k0.as<uint64_t>());
+    launch(build_chunk_kernel, grid_for(n, 256), 256, 0, stream(), plan, nullptr, n, chunk, k0.as<uint64_t>());
     CUDA_CHECK(cudaMemsetAsync(hist.p, 0, hist.bytes, stream()));
-    hist8_kernel<<<grid_for(n, 256 * 8), 256, 0, stream()>>>(k0.as<uint64_t>(), n, 8, hist.as<unsigned long long>());
-    CUDA_CHECK(cudaGetLastError());
-    count_launch(2);
+    launch(hist8_kernel, grid_for(n, 256 * 8), 256, 0, stream(), k0.as<uint64_t>(), n, 8, hist.as<unsigned long long>());
     std::vector<unsigned long long> h(8 * 256);
     d2h(h.data(), hist.p, h.size());
     sync();
@@ -626,18 +597,14 @@ static Table* top_n_select(const Table* t, const b2_order_by_arg* keys, int nkey
       if (d == 0 || tied <= 8192) { thr = pval | (d > 0 ? (1ull << (8 * d)) - 1 : 0); m = below + tied; break; }
       d--;
       CUDA_CHECK(cudaMemsetAsync(hist.p, 0, 256 * 8, stream()));
-      hist_prefix_kernel<<<grid_for(n, 256 * 8), 256, 0, stream()>>>(k0.as<uint64_t>(), n, pmask, pval, 8 * d, hist.as<unsigned long long>());
-      CUDA_CHECK(cudaGetLastError());
-      count_launch();
+      launch(hist_prefix_kernel, grid_for(n, 256 * 8), 256, 0, stream(), k0.as<uint64_t>(), n, pmask, pval, 8 * d, hist.as<unsigned long long>());
       d2h(hd.data(), hist.p, 256);
       sync();
     }
   }
   if (m < 0 || m > n / 4) return nullptr;   // all leading bytes equal, or one value dominates: sort everything
   ColGuard mask(new_column(B2_BOOL8, 0, n, false));
-  topn_mask_kernel<<<grid_for(n, 256), 256, 0, stream()>>>(k0.as<uint64_t>(), n, thr, mask.c->data.as<int8_t>());
-  CUDA_CHECK(cudaGetLastError());
-  count_launch();
+  launch(topn_mask_kernel, grid_for(n, 256), 256, 0, stream(), k0.as<uint64_t>(), n, thr, mask.c->data.as<int8_t>());
   std::unique_ptr<Table, void (*)(Table*)> sub(filter_by_mask(t, mask.c), table_release);
   if (sub->rows < std::min<int64_t>(limit, n)) throw Error(B2_ERR_INVALID, "top-n selection lost rows");
   DevBuf perm = sort_order(sub.get(), keys, nkeys);
@@ -713,11 +680,7 @@ int b2_search_bounds(b2_handle sorted_table, b2_handle values_table, const b2_or
   }
   SortPlan sp = make_sort_plan(st, k.data(), nkeys, true), vp = make_sort_plan(vt, k.data(), nkeys, true);
   ColGuard out(new_column(B2_INT32, 0, vt->rows, false));
-  if (vt->rows) {
-    bounds_kernel<<<grid_for(vt->rows, 128), 128, 0, stream()>>>(sp, vp, st->rows, vt->rows, upper, out.c->data.as<int32_t>());
-    CUDA_CHECK(cudaGetLastError());
-    count_launch();
-  }
+  if (vt->rows) launch(bounds_kernel, grid_for(vt->rows, 128), 128, 0, stream(), sp, vp, st->rows, vt->rows, upper, out.c->data.as<int32_t>());
   *out_int32_idx = to_handle(out.release());
   B2_CATCH
 }
