@@ -17,6 +17,7 @@
 //     lane per group per warp touches the accumulator; CTAs merge into the global table once.
 //   * global open-addressing table (any cardinality): insert by CAS on a representative row index,
 //     key equality against that row, RED/ATOM on per-slot accumulators.
+#include "partition.cuh"
 #include "prim.cuh"
 #include "rowops.cuh"
 #include "vm.cuh"
@@ -785,6 +786,190 @@ __global__ void rg_offsets_kernel(const uint32_t* __restrict__ h, int64_t n, uin
   }
 }
 
+// ---- fused materialise + first radix pass (plans without a predicate: every row is kept, so a row's tile is known up front) --
+// A count pass takes the first digit straight from the key columns (part_tile_hist_kernel with RGKeyDigit), and ONE kernel
+// then evaluates the projection and writes every materialised array already in first-digit order: the rows never land in
+// HBM in input order only to be read back by the first scatter pass.  The tile is FS_TILE = 2048 rows for both kernels (the
+// VM runs over the same tile, so its output registers ARE the tile's value copy): one 32 KB stage buffer (2048 x the widest
+// array, 16 B) next to the VM's registers leaves room for two CTAs (16 warps) per SM.
+constexpr int FS_STEPS = 8, FS_TILE = PT_NT * FS_STEPS, FS_WARP_ITEMS = FS_TILE / PS_WARPS, FS_STAGE_BYTES = FS_TILE * 16;
+static_assert(PT_NT == VM_NT, "the fused kernel runs the VM with the scatter's threads");
+struct RGKeyDigit {   // keys packed and hashed exactly as radix_rows_kernel does; digit = low `bits` of the stored 32-bit hash
+  KeyCols keys;
+  int32_t key_shift[MAX_KEYS];
+  uint32_t mask;
+  __device__ __forceinline__ void pack(int64_t i, uint64_t& k0, uint64_t& k1) const {
+    u128 bits = 0;
+    for (int k = 0; k < keys.n; k++) bits |= (u128)key_bits(keys.c[k], i) << key_shift[k];
+    k0 = (uint64_t)bits; k1 = (uint64_t)(bits >> 64);
+  }
+  __device__ __forceinline__ int32_t operator()(int64_t i) const {
+    uint64_t k0, k1;
+    pack(i, k0, k1);
+    return (int32_t)((uint32_t)(rg_hash(k0, k1) >> 32) & mask);
+  }
+};
+
+// one integer key column of a warp's FS_STEPS x 32 rows, zero-extended into the packed keys as key_bits does.  Every load of
+// the column is issued before the first one is used: a per-row walk over the key columns (RGKeyDigit::pack) waits for each
+// load in turn, one memory latency per row and column at the two CTAs per SM this kernel runs
+template <typename T>
+__device__ __forceinline__ void fs_key_col(const void* data, int64_t wbase, int64_t nrows, int shift, u128 (&bits)[FS_STEPS]) {
+  const int lane = threadIdx.x & 31;
+  T x[FS_STEPS];
+#pragma unroll
+  for (int r = 0; r < FS_STEPS; r++) {
+    const int64_t i = wbase + r * 32 + lane;
+    x[r] = i < nrows ? reinterpret_cast<const T*>(data)[i] : (T)0;
+  }
+#pragma unroll
+  for (int r = 0; r < FS_STEPS; r++) bits[r] |= (u128)x[r] << shift;
+}
+
+__global__ void __launch_bounds__(VM_NT, 2) radix_rows_scatter_kernel(const VMProgramHeader* __restrict__ g_hdr, const VMInstr* __restrict__ g_code,
+                                                                      const __grid_constant__ VMInputs in, const __grid_constant__ RGPlan rp,
+                                                                      const __grid_constant__ RGKeyDigit kd, RGRows rows, int64_t nrows,
+                                                                      int64_t ntiles, const int32_t* __restrict__ base) {
+  __shared__ VMShared sh;
+  __shared__ uint32_t s_wh[PS_WARPS][256];
+  __shared__ int32_t s_start[257], s_gbase[256];
+  __shared__ uint8_t s_owner[FS_TILE];
+  __shared__ uint16_t s_pos[FS_TILE];                 // tile row -> its place in the tile's partition order
+  extern __shared__ __align__(16) char fs_dyn[];      // stage buffer (FS_STAGE_BYTES), then the VM registers
+  char* stage = fs_dyn;
+  const RInstr* code = vm_load_program(sh, g_hdr, g_code, in, fs_dyn + FS_STAGE_BYTES, nullptr, nullptr, FS_TILE);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int nparts = (int)kd.mask + 1;
+  for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    const int tile_n = (int)min((int64_t)FS_TILE, nrows - tile * FS_TILE);
+    for (int k = threadIdx.x; k < PS_WARPS * 256; k += PT_NT) (&s_wh[0][0])[k] = 0;
+    __syncthreads();
+    // 1. keys of this warp's 256 rows (all loads before the first use), ranked 32 at a time with match_any as in part_scatter2
+    const int64_t wbase = tile * FS_TILE + (int64_t)warp * FS_WARP_ITEMS;
+    uint64_t k0[FS_STEPS], k1[FS_STEPS];
+    uint8_t pid[FS_STEPS];
+    uint16_t lpos[FS_STEPS];
+    {
+      u128 bits[FS_STEPS];
+#pragma unroll
+      for (int r = 0; r < FS_STEPS; r++) bits[r] = 0;
+      for (int k = 0; k < kd.keys.n; k++) {
+        const KeyCol& c = kd.keys.c[k];
+        const int sh = kd.key_shift[k];
+        if (c.dtype == B2_FLOAT32 || c.dtype == B2_FLOAT64) {   // NaN / -0.0 normalisation: key_bits row by row
+#pragma unroll
+          for (int r = 0; r < FS_STEPS; r++) {
+            const int64_t i = wbase + r * 32 + lane;
+            if (i < nrows) bits[r] |= (u128)key_bits(c, i) << sh;
+          }
+        } else switch (c.width) {
+          case 1: fs_key_col<uint8_t>(c.data, wbase, nrows, sh, bits); break;
+          case 2: fs_key_col<uint16_t>(c.data, wbase, nrows, sh, bits); break;
+          case 4: fs_key_col<uint32_t>(c.data, wbase, nrows, sh, bits); break;
+          default: fs_key_col<uint64_t>(c.data, wbase, nrows, sh, bits); break;
+        }
+      }
+#pragma unroll
+      for (int r = 0; r < FS_STEPS; r++) { k0[r] = (uint64_t)bits[r]; k1[r] = (uint64_t)(bits[r] >> 64); }
+    }
+#pragma unroll
+    for (int r = 0; r < FS_STEPS; r++) {
+      const bool in_range = wbase + r * 32 + lane < nrows;
+      const uint32_t d = in_range ? ((uint32_t)(rg_hash(k0[r], k1[r]) >> 32) & kd.mask) : 256u + lane;   // out-of-range lanes match nobody
+      const uint32_t m = __match_any_sync(0xffffffffu, d);
+      const uint32_t before = __popc(m & ((1u << lane) - 1u));
+      uint32_t prev = 0;
+      if (in_range) prev = s_wh[warp][d];
+      __syncwarp();
+      if (in_range && before == 0) s_wh[warp][d] = prev + __popc(m);
+      __syncwarp();
+      pid[r] = (uint8_t)d;
+      lpos[r] = (uint16_t)(prev + before);
+    }
+    __syncthreads();
+    {  // partition d = threadIdx.x: exclusive offsets of the warps inside the partition's run, run length, global base
+      const int d = threadIdx.x;
+      uint32_t run = 0;
+#pragma unroll
+      for (int w = 0; w < PS_WARPS; w++) { const uint32_t c = s_wh[w][d]; s_wh[w][d] = run; run += c; }
+      s_start[d + 1] = (int32_t)run;
+      s_gbase[d] = d < nparts ? base[(int64_t)d * ntiles + tile] : 0;
+    }
+    __syncthreads();
+    if (threadIdx.x < 32) {   // exclusive scan of the 256 run lengths (8 per lane)
+      int32_t c[8], sum = 0;
+#pragma unroll
+      for (int k = 0; k < 8; k++) { c[k] = s_start[lane * 8 + k + 1]; sum += c[k]; }
+      int32_t inc = sum;
+      for (int o = 1; o < 32; o <<= 1) { const int32_t t = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += t; }
+      int32_t runx = inc - sum;
+#pragma unroll
+      for (int k = 0; k < 8; k++) { s_start[lane * 8 + k] = runx; runx += c[k]; }
+      if (lane == 31) s_start[256] = runx;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int r = 0; r < FS_STEPS; r++) {
+      if (wbase + r * 32 + lane < nrows) {
+        const int p = pid[r];
+        lpos[r] = (uint16_t)(s_start[p] + s_wh[warp][p] + lpos[r]);
+        s_owner[lpos[r]] = (uint8_t)p;
+        s_pos[warp * FS_WARP_ITEMS + r * 32 + lane] = lpos[r];
+      }
+    }
+    // 2. hash and key words, staged from registers in partition order (ps_store ends with a barrier)
+    uint32_t* st32 = reinterpret_cast<uint32_t*>(stage);
+    uint64_t* st64 = reinterpret_cast<uint64_t*>(stage);
+#pragma unroll
+    for (int r = 0; r < FS_STEPS; r++)
+      if (wbase + r * 32 + lane < nrows) st32[lpos[r]] = (uint32_t)(rg_hash(k0[r], k1[r]) >> 32);
+    __syncthreads();
+    ps_store<uint32_t, FS_TILE>(rows.h, st32, tile_n, s_owner, s_start, s_gbase);
+#pragma unroll
+    for (int r = 0; r < FS_STEPS; r++)
+      if (wbase + r * 32 + lane < nrows) st64[lpos[r]] = k0[r];
+    __syncthreads();
+    ps_store<uint64_t, FS_TILE>(rows.k0, st64, tile_n, s_owner, s_start, s_gbase);
+    if (rp.has_k1) {
+#pragma unroll
+      for (int r = 0; r < FS_STEPS; r++)
+        if (wbase + r * 32 + lane < nrows) st64[lpos[r]] = k1[r];
+      __syncthreads();
+      ps_store<uint64_t, FS_TILE>(rows.k1, st64, tile_n, s_owner, s_start, s_gbase);
+    }
+    // 3. the projection over the same tile; each value array is staged from the VM's output registers in partition order
+    VMCtx cx = vm_ctx(&sh.hdr, &in, fs_dyn + FS_STAGE_BYTES, tile, nrows);
+    vm_run(tile_info(cx), code, 0, sh.hdr.ninstr);
+    for (int s = 0; s < rp.nvals; s++) {
+      const Opnd op = resolve(cx, sh.hdr.outs[rp.val[s].out_idx], mt_width(rp.val[s].in_mt));
+      const int mt = rp.val[s].in_mt;
+#pragma unroll
+      for (int j = 0; j < FS_STEPS; j++) {
+        const int i = threadIdx.x + j * VM_NT;
+        const int64_t g = cx.tile_base + i;
+        if (g >= nrows) continue;
+        const bool valid = opnd_valid(op, i, g);
+        const int k = s_pos[i];
+        if (rp.val[s].width == 16) {
+          reinterpret_cast<i128*>(stage)[k] = valid ? opnd_ld<i128>(op, i) : (i128)0;
+        } else {
+          int64_t x = 0;
+          if (valid) switch (mt) {
+            case MT_I8: x = opnd_ld<int8_t>(op, i); break;
+            case MT_I16: x = opnd_ld<int16_t>(op, i); break;
+            case MT_I32: x = opnd_ld<int32_t>(op, i); break;
+            default: x = opnd_ld<int64_t>(op, i); break;
+          }
+          reinterpret_cast<int64_t*>(stage)[k] = x;
+        }
+      }
+      __syncthreads();
+      if (rp.val[s].width == 16) ps_store<uint4, FS_TILE>(reinterpret_cast<uint4*>(rows.v[s]), reinterpret_cast<const uint4*>(stage), tile_n, s_owner, s_start, s_gbase);
+      else ps_store<uint64_t, FS_TILE>(reinterpret_cast<uint64_t*>(rows.v[s]), st64, tile_n, s_owner, s_start, s_gbase);
+    }
+  }
+}
+
 struct RGAgg {
   RGRows rows;
   const int32_t* off;
@@ -1378,7 +1563,22 @@ static Table* radix_groupby(const Program* prog, const Table* t, const AggPlan& 
   }
   if (C < 1024) return nullptr;
 
-  // 1. materialise the (filtered, projected) rows
+  // P: radix partitions such that a partition's groups fit the shared-memory table at load <= ~0.4
+  auto parts_for = [&](int64_t rows) { int64_t p = 1; while (p * (int64_t)(C * 2 / 5) < rows && p < (1 << 20)) p <<= 1; return p; };
+  // Without a predicate every row is kept, so the first radix pass can be fused into the materialisation (count pass from the
+  // key columns, then radix_rows_scatter_kernel).  B2_AGG_NO_FUSED_FIRST_PASS forces the separate materialise + passes.
+  const int fs_smem = FS_STAGE_BYTES + prog->hdr.bytes_per_row * FS_TILE;
+  bool fused = !plan.has_pred && !rp.use_vbits && parts_for(n) > 1 && !getenv("B2_AGG_NO_FUSED_FIRST_PASS");
+  if (fused) {
+    int dev = 0, optin = 0;
+    CUDA_CHECK(cudaGetDevice(&dev));
+    CUDA_CHECK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+    cudaFuncAttributes fa;
+    CUDA_CHECK(cudaFuncGetAttributes(&fa, radix_rows_scatter_kernel));
+    fused = fs_smem + (int)fa.sharedSizeBytes <= optin;
+  }
+
+  // 1. materialise the (filtered, projected) rows; the fused path also does the first radix pass
   struct Side { DevBuf h, k0, k1, v[RG_MAX_VALS], vbits; };
   Side A, B;
   auto alloc_side = [&](Side& sd) {
@@ -1396,24 +1596,42 @@ static Table* radix_groupby(const Program* prog, const Table* t, const AggPlan& 
   alloc_side(A);
   DevBuf counter(16);
   CUDA_CHECK(cudaMemsetAsync(counter.p, 0, 16, stream()));
-  {
+  int64_t m = n, P = 1;
+  int lgP = 0, shift = 0;   // shift: hash bits already sorted by
+  DevBuf fs_cnt, fs_sums;   // freed at the end of the call, after the sync that waits for the kernels reading them
+  if (fused) {
+    P = parts_for(n);
+    while ((1LL << lgP) < P) lgP++;
+    shift = std::min(8, lgP);
+    RGKeyDigit kd; memset(&kd, 0, sizeof(kd));
+    kd.keys = plan.keys; kd.keys.n = nkeys;
+    for (int k = 0; k < nkeys; k++) kd.key_shift[k] = rp.key_shift[k];
+    kd.mask = (1u << shift) - 1u;
+    const int64_t ntiles = (n + FS_TILE - 1) / FS_TILE, cells = ntiles << shift;
+    fs_cnt = DevBuf((size_t)(cells + 1) * 4);
+    launch("part_tile_hist_kernel(keys)", part_tile_hist_kernel<RGKeyDigit, FS_STEPS>, (int)ntiles, PT_NT, 0, stream(), kd, n, (int32_t)(1 << shift),
+           ntiles, fs_cnt.as<int32_t>());
+    fs_sums = exclusive_scan<int32_t, int32_t>(fs_cnt.as<int32_t>(), fs_cnt.as<int32_t>(), cells, true);
+    // one tile per CTA and pass while every CTA is resident; a wider program (fewer CTAs per SM) loops over tiles
+    const int grid = (int)std::min<int64_t>(ntiles, (int64_t)sm_count() * 2);
+    launch("radix_rows_scatter_kernel", radix_rows_scatter_kernel, grid, VM_NT, fs_smem, stream(), prog->d_hdr.as<VMProgramHeader>(),
+           prog->d_code.as<VMInstr>(), in, rp, kd, rows_of(A), n, ntiles, fs_cnt.as<int32_t>());
+  } else {
     const int vm_smem = prog->hdr.smem_bytes;
     launch("radix_rows_kernel", radix_rows_kernel, vm_grid(n, vm_smem, prog->hdr.tile_rows), VM_NT, vm_smem, stream(), prog->d_hdr.as<VMProgramHeader>(),
            prog->d_code.as<VMInstr>(), in, plan, rp, rows_of(A), n, counter.as<unsigned long long>());
+    if (plan.has_pred) { unsigned long long hm = 0; d2h(&hm, counter.p, 1); sync(); m = (int64_t)hm; }
+    if (m == 0) return nullptr;
+    // 2. radix partition by key hash
+    P = parts_for(m);
+    while ((1LL << lgP) < P) lgP++;
   }
-  int64_t m = n;
-  if (plan.has_pred) { unsigned long long hm = 0; d2h(&hm, counter.p, 1); sync(); m = (int64_t)hm; }
-  if (m == 0) return nullptr;
-  // 2. radix partition by key hash so that a partition's groups fit the shared-memory table at load <= ~0.4
-  int64_t P = 1;
-  while (P * (int64_t)(C * 2 / 5) < m && P < (1 << 20)) P <<= 1;
-  int lgP = 0; while ((1LL << lgP) < P) lgP++;
   Side* cur = &A; Side* oth = &B;
-  if (P > 1) {
+  if (shift < lgP) {
     alloc_side(B);
     // LSD passes of at most 8 bits each (the <= 256-way scatter is the fast one), stable, so the final order is by h & (P - 1);
     // each pass takes its digit straight from the hash array it moves
-    for (int shift = 0; shift < lgP;) {
+    while (shift < lgP) {
       const int bits = std::min(8, lgP - shift);
       ScatterCols sc; memset(&sc, 0, sizeof(sc));
       auto add = [&](DevBuf& i, DevBuf& o, int w) { sc.width[sc.n] = w; sc.in[sc.n] = i.p; sc.out[sc.n] = o.p; sc.n++; };

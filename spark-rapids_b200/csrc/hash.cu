@@ -9,7 +9,7 @@
 // One kernel hashes all key columns (chained: the hash of column i seeds column i+1; a NULL leaves
 // the running hash unchanged), applies pmod and writes the partition id; Table.partition is then a
 // stable one- or two-digit radix split (sort.cu) followed by the fused multi-column gather.
-#include "pack16.cuh"
+#include "partition.cuh"
 #include "prim.cuh"
 #include "rowops.cuh"
 #include "murmur.cuh"
@@ -50,7 +50,7 @@ Table* gather_table(const Table* t, const int32_t* d_map, int64_t n, bool nullif
 // shared memory, 256 rows at a time in row order) and writes each fixed-width NOT NULL column straight to its final
 // place.  Reads are coalesced, writes are coalesced per run of equal ids.  Other columns (strings, nullable) go
 // through the gather map the same kernel can emit.  Replaces id->key expansion + radix pass + random-read gather.
-constexpr int PT_NT = 256, PT_STEPS = 16, PT_TILE = PT_NT * PT_STEPS, PT_MAXP = 1024;   // PT_MAXC, ScatterCols: prim.cuh
+// PT_NT, PT_TILE, part_tile_hist_kernel, ps_store: partition.cuh
 // Where a row's partition id comes from: an id array (Table.partition), or a digit of a 32-bit hash array (the radix group-by's
 // passes, which move that hash array anyway: no separate digit pass and no id array)
 struct PidArray {
@@ -64,21 +64,6 @@ struct HashDigit {
   // default cache policy: the scatter moves the hash array itself right after, and that read should hit L2
   __device__ __forceinline__ int32_t operator()(int64_t i) const { return (int32_t)((h[i] >> shift) & mask); }
 };
-
-template <typename Pid>
-__global__ void __launch_bounds__(PT_NT) part_tile_hist_kernel(const Pid pids, int64_t n, int32_t nparts, int64_t ntiles,
-                                                               int32_t* __restrict__ tile_cnt) {
-  __shared__ int32_t h[PT_MAXP];
-  for (int p = threadIdx.x; p < nparts; p += PT_NT) h[p] = 0;
-  __syncthreads();
-  const int64_t tile = blockIdx.x;
-  for (int j = 0; j < PT_STEPS; j++) {
-    const int64_t i = tile * PT_TILE + (int64_t)j * PT_NT + threadIdx.x;
-    if (i < n) { const int32_t p = pids(i); if ((uint32_t)p < (uint32_t)nparts) atomicAdd(&h[p], 1); }
-  }
-  __syncthreads();
-  for (int p = threadIdx.x; p < nparts; p += PT_NT) tile_cnt[(int64_t)p * ntiles + tile] = h[p];
-}
 
 __global__ void __launch_bounds__(PT_NT) part_scatter_kernel(const int32_t* __restrict__ pids, int64_t n, int32_t nparts, int64_t ntiles,
                                                              const int32_t* __restrict__ base, const __grid_constant__ ScatterCols sc,
@@ -131,7 +116,7 @@ __global__ void __launch_bounds__(PT_NT) part_scatter_kernel(const int32_t* __re
 // per-warp running counts (no block barrier inside the loop), one cross-warp scan gives every row its position in the
 // tile's partition-sorted order.  Each array is then staged through shared memory in that order, so a partition's run
 // leaves the SM as consecutive addresses (full sectors) instead of one scattered 8-byte store per row.
-constexpr int PS_WARPS = PT_NT / 32, PS_WARP_ITEMS = PT_TILE / PS_WARPS;
+constexpr int PS_WARP_ITEMS = PT_TILE / PS_WARPS;
 template <typename T>
 __device__ __forceinline__ void ps_move(const T* __restrict__ in, T* __restrict__ out, T* stage, const uint16_t* lpos, int64_t wbase, int64_t n, int tile_n,
                                         const uint8_t* s_owner, const int32_t* s_start, const int32_t* s_gbase) {
@@ -142,43 +127,7 @@ __device__ __forceinline__ void ps_move(const T* __restrict__ in, T* __restrict_
     if (i < n) stage[lpos[r]] = __ldcs(&in[i]);   // read once: evict-first, so the stream does not push the partially written sectors out of L2
   }
   __syncthreads();
-  // Every store that can be is a 16-byte store to a 16-byte aligned DESTINATION: the vector slot anchored at stage index k0
-  // is shifted back by the run's misalignment s = dest(k0) % V, so it reads V (unaligned) elements from shared memory and
-  // writes one aligned vector.  Only the elements whose aligned destination vector crosses the run's ends (< 2V per run)
-  // leave one by one.  (The first version stored aligned STAGE vectors and fell back to per-element loops for whole
-  // misaligned runs: the profiler counted about twice the ideal store sectors and DRAM writes.)
-  constexpr int V = sizeof(T) >= 16 ? 1 : 16 / (int)sizeof(T);
-  // fixed trip count, fully unrolled: the iterations are independent and their shared-memory loads and global stores overlap.
-  // (With the runtime bound `k0 < tile_n` the compiler unrolled this loop in one build and not in the next, and the kernel's
-  // speed changed with an unrelated header change.)
-  constexpr int ITERS = PT_TILE / (PT_NT * V);
-#pragma unroll
-  for (int it = 0; it < ITERS; it++) {
-    const int k0 = (it * PT_NT + (int)threadIdx.x) * V;
-    if (k0 >= tile_n) continue;
-    if (V == 1) { const int p = s_owner[k0]; __stcs(&out[(int64_t)s_gbase[p] + (k0 - s_start[p])], stage[k0]); continue; }
-    {
-      const int p = s_owner[k0];
-      const int64_t c = (int64_t)s_gbase[p] - s_start[p];       // dest(k) = k + c inside run p
-      const int kk = k0 - (int)((k0 + c) % V);
-      if (kk >= s_start[p] && kk + V <= s_start[p + 1]) {
-        // whole sectors, never touched again: streaming store.  The boundary elements below keep the default policy: their
-        // sector is completed by the neighbouring tile's run, and the kernel's DRAM writes depend on those half-written
-        // sectors still being in L2 when the other half arrives
-        __stcs(reinterpret_cast<uint4*>(out + (kk + c)), pack16<T>(stage + kk));
-      }
-    }
-#pragma unroll
-    for (int i = 0; i < V; i++) {
-      const int e = k0 + i;
-      if (e >= tile_n) break;
-      const int q = s_owner[e];
-      const int64_t c = (int64_t)s_gbase[q] - s_start[q];
-      const int kk = e - (int)((e + c) % V);
-      if (!(kk >= s_start[q] && kk + V <= s_start[q + 1])) out[e + c] = stage[e];
-    }
-  }
-  __syncthreads();
+  ps_store<T, PT_TILE>(out, stage, tile_n, s_owner, s_start, s_gbase);
 }
 __global__ void __launch_bounds__(PT_NT, 4) part_scatter2_kernel(const HashDigit pids, int64_t n, int32_t nparts, int64_t ntiles,
                                                               const int32_t* __restrict__ base, const __grid_constant__ ScatterCols sc) {

@@ -958,13 +958,16 @@ struct VMShared {
 // cooperative load: header into shared memory, then one thread per instruction resolves its operands
 static __device__ __forceinline__ const RInstr* vm_load_program(VMShared& sh, const VMProgramHeader* g_hdr, const VMInstr* g_code,
                                                                  const VMInputs& in, char* regs, const VMStage* stage = nullptr,
-                                                                 char* stage_base = nullptr) {
+                                                                 char* stage_base = nullptr, int fixed_tile_rows = 0) {
   const int* src = reinterpret_cast<const int*>(g_hdr);
   int* dst = reinterpret_cast<int*>(&sh.hdr);
   for (int k = threadIdx.x; k < (int)(sizeof(VMProgramHeader) / 4); k += blockDim.x) dst[k] = src[k];
   __syncthreads();
-  if (stage && stage->n > 0) {   // the staged kernel picks its own tile size (registers + two stage buffers per tile)
-    if (threadIdx.x == 0) { sh.hdr.tile_rows = stage->tile_rows; sh.hdr.smem_bytes = sh.hdr.bytes_per_row * stage->tile_rows; }
+  // the staged kernel picks its own tile size (registers + two stage buffers per tile); a kernel whose tile is fixed by
+  // something else (the radix group-by's fused first pass) passes it as fixed_tile_rows (a multiple of VM_NT, <= 4096)
+  const int own_rows = (stage && stage->n > 0) ? stage->tile_rows : fixed_tile_rows;
+  if (own_rows > 0) {
+    if (threadIdx.x == 0) { sh.hdr.tile_rows = own_rows; sh.hdr.smem_bytes = sh.hdr.bytes_per_row * own_rows; }
     __syncthreads();
   }
   const int n = sh.hdr.ninstr;
