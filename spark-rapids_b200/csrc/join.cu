@@ -632,7 +632,8 @@ int b2_join_probe_sel(b2_handle ht, b2_handle probe_keys_table, b2_handle select
     return B2_OK;
   }
   B2_CHECK(kind >= B2_JOIN_INNER && kind <= B2_JOIN_LEFT_ANTI, "bad join kind");
-  const int64_t n = sel ? nsel : pt->rows;
+  // an empty selection vector has no data buffer (sel == nullptr) and selects no row
+  const int64_t n = selection ? nsel : pt->rows;
   const bool semi_like = kind == B2_JOIN_LEFT_SEMI || kind == B2_JOIN_LEFT_ANTI;
   KeyCols pk = key_cols_of(pt, jt->key_idx.data(), (int)jt->key_idx.size());
   KeyCols bk = key_cols_of(jt->keys, jt->key_idx.data(), (int)jt->key_idx.size());

@@ -6,6 +6,9 @@ import operator
 import numpy as np
 import pytest
 
+from oracle import spark_cpu as O
+from tests.test_join_paths_gpu import join_maps
+
 pytestmark = pytest.mark.gpu
 
 FUSED, SEL_FILTER, SEL_PROBE = "join_filter_probe_kernel", "simple_filter_ids_kernel", "join_probe_distinct1_kernel"
@@ -13,19 +16,11 @@ TILE = 8192                      # rows per tile of the fused kernel
 OPS = [operator.eq, operator.ne, operator.lt, operator.le, operator.gt, operator.ge]
 
 
-def ref_pairs(skey, svalid, keep, bkey, bvalid):
-    """numpy: (stream row, build row) for every passing stream row and build row with equal non-NULL keys, sorted"""
-    bi = np.flatnonzero(bvalid)
-    order = bi[np.argsort(bkey[bi], kind="stable")]
-    bs = bkey[order]
-    rows = np.flatnonzero(keep & svalid)
-    lo = np.searchsorted(bs, skey[rows], "left")
-    hi = np.searchsorted(bs, skey[rows], "right")
-    cnt = hi - lo
-    left = np.repeat(rows, cnt)
-    start = np.repeat(lo - np.concatenate(([0], np.cumsum(cnt)[:-1])), cnt)
-    right = order[start + np.arange(len(left))] if len(left) else np.zeros(0, np.int64)
-    return sorted(zip(left.tolist(), right.tolist()))
+def passing_pairs(skey, svalid, keep, bkey, bvalid):
+    """sorted (stream row, build row) pairs of the passing stream rows, from the exact reference (test_join_paths_gpu)"""
+    rows = np.flatnonzero(keep)
+    lm, rm = join_maps([O.OCol(bkey, bvalid, (O.INT64, 0, 0))], [O.OCol(skey[rows], svalid[rows], (O.INT64, 0, 0))], 0)
+    return sorted(zip(rows[lm].tolist(), rm.tolist()))
 
 
 def pairs_of(lm, rm):
@@ -49,7 +44,7 @@ def check(b2, stream_cols, key_col, pred, keep, bkey, bvalid=None, skey_valid=No
     assert (FUSED in names) == fused, names
     if fused:
         assert SEL_FILTER not in names and SEL_PROBE not in names, names
-    want = ref_pairs(skey.astype(np.int64), svalid, keep, bkey.astype(np.int64), bvalid)
+    want = passing_pairs(skey.astype(np.int64), svalid, keep, bkey.astype(np.int64), bvalid)
     got = pairs_of(lm, rm)
     assert npass == int(keep.sum())
     assert len(lm) == len(want)
@@ -198,7 +193,7 @@ def test_odd_offset_slice(b2):
     assert FUSED in names, names
     keep = d[1:] >= 40
     assert npass == int(keep.sum())
-    assert pairs_of(lm, rm) == ref_pairs(skey[1:], np.ones(n, bool), keep, bkey, np.ones(len(bkey), bool))
+    assert pairs_of(lm, rm) == passing_pairs(skey[1:], np.ones(n, bool), keep, bkey, np.ones(len(bkey), bool))
 
 
 def test_exec_path_several_batches(b2):
