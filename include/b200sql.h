@@ -303,6 +303,12 @@ int b2_hash_partition(b2_handle table, const int32_t* key_cols, int32_t nkeys, i
 int b2_partition_by_ids(b2_handle table, b2_handle int32_part_ids, int32_t num_partitions,
                         b2_handle* out_table, int32_t* offsets_out);  /* Table.partition */
 int b2_slice(b2_handle table, int64_t start, int64_t end, b2_handle* out_table); /* contiguousSplit piece */
+/* GpuBatchSubPartitioner (GpuSubPartitionHashJoin.scala:86-221: hashPartition + contiguousSplit) in one pass: rows of `table`
+ * (or only the rows of the INT32 selection vector `sel`, 0 = all rows) split into num_parts tables by
+ * pmod(murmur3(key columns, seed), num_parts); each output owns its buffers, keeps the rows' input order and holds the columns
+ * keep_cols (NULL = all, in that order); out_tables[p] = 0 when part p is empty.  2 <= num_parts <= 256. */
+int b2_hash_split(b2_handle table, b2_handle sel, const int32_t* key_cols, int32_t nkeys, int32_t seed, int32_t num_parts,
+                  const int32_t* keep_cols, int32_t nkeep, b2_handle* out_tables);
 
 /* ---- a10: Parquet -> device (GpuParquetScan.scala:2089-2127 readPartFile, :3322-3503) ---------- */
 /* host_buf is the reassembled mini-file "PAR1 + column chunks + footer + len + PAR1" exactly as
@@ -432,6 +438,15 @@ int b2_exec_shuffled_hash_join_select(b2_handle stream_child, b2_handle build_ch
  * equi-matched pairs survive — Table.mixed{Inner,Left,LeftSemi,LeftAnti}JoinGatherMap(s) (GpuHashJoin.scala:335-600),
  * ConditionalHashJoinIterator (:1556).  Inner / left outer / left semi / left anti. */
 int b2_exec_join_set_condition(b2_handle join, b2_handle condition_program);
+/* GpuSubPartitionHashJoin (GpuShuffledHashJoinExec.scala:228-281, GpuSubPartitionHashJoin.scala:86-617): when the build side
+ * passes target_bytes (table_bytes; raised to 16 KiB) both sides are split into num_partitions (2..256; Spark default 16,
+ * RapidsConf.scala:2660) spillable buckets by murmur3 seed 100 of the join keys and joined bucket by bucket; adjacent small
+ * buckets are packed up to the target, a bucket still over it (FULL OUTER: by its build or its stream side) is split once
+ * more (seed 110) and then joined as it is, so the rows of a single key must fit on the device.  Without this call, or when the build side stays within target_bytes,
+ * the join is unchanged. */
+int b2_exec_join_set_sub_partitioning(b2_handle join, int64_t target_bytes, int32_t num_partitions);
+/* out4: first-level buckets (0 = not sub-partitioned), buckets repartitioned, build bytes split, stream bytes split */
+int b2_exec_join_sub_partition_stats(b2_handle join, int64_t* out4);
 /* GpuBroadcastExchangeExec (GpuBroadcastExchangeExec.scala): every rank gets the whole child relation, one batch.  Used as
  * the build child of a join it makes GpuBroadcastHashJoinExec (GpuBroadcastHashJoinExecBase.scala:1-203). */
 int b2_exec_broadcast_exchange(b2_handle child, b2_handle comm, int32_t rank, int32_t world, b2_handle* out);

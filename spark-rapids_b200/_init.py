@@ -602,6 +602,16 @@ def hash_partition(table, key_cols, num_partitions, seed=42):
     return Table(out.value), list(offs)
 
 
+def hash_split(table, keys, seed, num_parts, sel=None, keep=None):
+    """rows of `table` (only those the INT32 selection vector `sel` names, when given) split by pmod(murmur3(keys, seed),
+    num_parts) -> list of num_parts Tables (None for an empty part) holding the columns `keep` (default all), rows in input order"""
+    out = (ctypes.c_int64 * num_parts)()
+    kp = None if keep is None else _i32s(keep)
+    check(lib.b2_hash_split(table.h, sel.h if sel is not None else 0, _i32s(keys), len(keys), seed, num_parts, kp,
+                            0 if keep is None else len(keep), out))
+    return [Table(h) if h else None for h in out]
+
+
 def partition_by_ids(table, part_ids, num_partitions):
     out = ctypes.c_int64()
     offs = (ctypes.c_int32 * (num_partitions + 1))()

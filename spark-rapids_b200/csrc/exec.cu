@@ -34,6 +34,8 @@ Table* filter_by_mask(const Table* t, Column* m);
 Column* rows_with_passing_pair(const Column* left_map, const Column* pass, int64_t stream_rows, bool invert);
 
 Table* slice_table(const Table* t, int64_t start, int64_t end);
+std::vector<Table*> hash_split_table(const Table* t, const int32_t* d_sel, int64_t n, const int32_t* key_cols, int nkeys, uint32_t seed,
+                                     int nparts, const std::vector<int>& keep);   // hash.cu
 
 // RmmRapidsRetryIterator.withRetry (RmmRapidsRetryIterator.scala:65-203): an allocation failure first spills (core.cu does
 // that inside the allocator) and surfaces as B2_ERR_OOM = GpuRetryOOM; the operator then makes everything spillable leave
@@ -69,6 +71,36 @@ struct TableRef {  // owning reference
 };
 
 static Table* from_handle_owned(b2_handle h) { return h ? reinterpret_cast<Table*>((intptr_t)h) : nullptr; }
+
+// A batch waiting in the spill store, with the facts about it that planning needs, so that planning never brings it back
+struct SpillPiece {
+  b2_handle sp = 0;
+  int64_t rows = 0, bytes = 0;
+  std::vector<int64_t> chars;    // per column: string bytes
+  std::vector<char> nullable;    // per column: carries validity
+  SpillPiece() {}
+  SpillPiece(const SpillPiece&) = delete;
+  SpillPiece(SpillPiece&& o) noexcept : sp(o.sp), rows(o.rows), bytes(o.bytes), chars(std::move(o.chars)), nullable(std::move(o.nullable)) { o.sp = 0; }
+  SpillPiece& operator=(SpillPiece&& o) noexcept {
+    if (this != &o) { close(); sp = o.sp; o.sp = 0; rows = o.rows; bytes = o.bytes; chars = std::move(o.chars); nullable = std::move(o.nullable); }
+    return *this;
+  }
+  ~SpillPiece() { close(); }
+  // registers `t` (the store takes its own reference)
+  void hold(const Table* t) {
+    rows = t->rows; bytes = table_bytes(t);
+    for (const Column* c : t->cols) { chars.push_back(c->dtype == B2_STRING ? c->chars_bytes : 0); nullable.push_back(c->nullable()); }
+    int rc = b2_spillable_create(to_handle(const_cast<Table*>(t)), &sp);
+    if (rc != B2_OK) throw Error(rc, b2_last_error());
+  }
+  void close() { if (sp) b2_spillable_close(sp); sp = 0; }
+  Table* get() const {
+    b2_handle h = 0;
+    int rc = b2_spillable_get(sp, &h);
+    if (rc != B2_OK) throw Error(rc, b2_last_error());
+    return from_handle_owned(h);
+  }
+};
 
 struct GpuExec {
   std::atomic<int> refs{1};
@@ -429,7 +461,11 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
   void build() {
     // prepareBuildBatchesForJoin: the whole build side becomes one batch
     std::vector<TableRef> parts;
-    while (true) { TableRef b(children[1]->next()); if (!b.t) break; parts.emplace_back(b.release()); }
+    if (sp_target > 0) {
+      if (hold_build_side(parts)) { built = true; return; }
+    } else {
+      while (true) { TableRef b(children[1]->next()); if (!b.t) break; parts.emplace_back(b.release()); }
+    }
     if (parts.empty()) throw Error(B2_ERR_UNSUPPORTED, "empty build side needs the build schema");
     if (parts.size() == 1) build_table = std::move(parts[0]);
     else { std::vector<const Table*> ts; for (auto& p : parts) ts.push_back(p.t); build_table = TableRef(concat_tables(ts)); }
@@ -502,6 +538,7 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
   Table* do_next() override {
     if (!todo.empty()) return drain_todo();
     if (!built) build();
+    if (sp_active) return sp_next();
     if (!fusion_checked) {
       fusion_checked = true;
       if (kind != B2_JOIN_FULL_OUTER && !condition && !getenv("B2_NO_FILTER_FUSION")) fused = dynamic_cast<GpuFilterExec*>(children[0]);
@@ -636,6 +673,214 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
     left.t->cols.clear(); right.t->cols.clear();
     return new_table(std::move(cols));
   }
+
+  // ---- GpuSubPartitionHashJoin (GpuSubPartitionHashJoin.scala) -------------------------------------------------------------
+  // Seeds 100 and 110, not the exchange's 42: rows reach this node already assigned by pmod(murmur3_42, world), and buckets by
+  // the same hash would leave only K / gcd(K, world) of the K buckets non-empty on each rank.
+  static constexpr int SP_SEED = 100, SP_RESEED = 110;
+  int64_t sp_target = 0;   // 0: off
+  int sp_parts = 16;
+  int64_t sp_stats[4] = {0, 0, 0, 0};
+  bool sp_active = false, sp_read = false;
+  struct Bucket {
+    std::vector<SpillPiece> build, stream;
+    int64_t build_bytes = 0, stream_bytes = 0;
+    bool resplit = false;   // made by repartitioning a bucket: never split again
+  };
+  std::deque<Bucket> sp_buckets;
+  std::deque<std::vector<SpillPiece>> sp_probe;   // the open pair's stream pieces, one group per probe batch
+  TableRef sp_build_empty, sp_stream_empty;       // zero-row tables of the carried columns
+  std::vector<int> sp_bkeys, sp_bkeep;            // first-level split of the build batches: keys and carried columns
+
+  // the columns one side carries through its buckets: with pruning and no condition the keys and the output columns (indices
+  // remapped), otherwise every column
+  std::vector<int> carried(int ncols, std::vector<int>& keys, std::vector<int>& out_cols) {
+    std::vector<int> keep;
+    if (!pruned || condition) { for (int c = 0; c < ncols; c++) keep.push_back(c); return keep; }
+    auto pos = [&](int c) {
+      if (c < 0 || c >= ncols) throw Error(B2_ERR_INVALID, "join column index out of range");
+      for (size_t k = 0; k < keep.size(); k++) if (keep[k] == c) return (int)k;
+      keep.push_back(c);
+      return (int)keep.size() - 1;
+    };
+    for (int& k : keys) k = pos(k);
+    for (int& c : out_cols) c = pos(c);
+    return keep;
+  }
+  static std::vector<TableRef> owned(std::vector<Table*>&& ts) {
+    std::vector<TableRef> out;
+    for (Table* t : ts) out.emplace_back(t);
+    return out;
+  }
+  template <typename BucketOf>
+  void split_into(const Table* t, const int32_t* d_sel, int64_t n, const std::vector<int>& keys, const std::vector<int>& keep, int seed, int nparts,
+                  BucketOf&& bucket_of, bool build_side, int64_t* bytes_out) {
+    std::vector<TableRef> parts = owned(with_retry([&] { return hash_split_table(t, d_sel, n, keys.data(), (int)keys.size(), (uint32_t)seed, nparts, keep); }));
+    for (int p = 0; p < nparts; p++) {
+      if (!parts[p].t) continue;
+      Bucket& b = bucket_of(p);
+      std::vector<SpillPiece>& dst = build_side ? b.build : b.stream;
+      dst.emplace_back();
+      dst.back().hold(parts[p].t);
+      (build_side ? b.build_bytes : b.stream_bytes) += dst.back().bytes;
+      if (bytes_out) *bytes_out += dst.back().bytes;
+    }
+  }
+  // Pulls the build side into the spill store.  False: it stayed within the target and `parts` holds its batches.  True: it
+  // passed the target and is split into the buckets.
+  bool hold_build_side(std::vector<TableRef>& parts) {
+    std::vector<SpillPiece> held;
+    int64_t bytes = 0;
+    auto first_level = [&](int p) -> Bucket& { return sp_buckets[p]; };
+    auto split = [&](const Table* t) { split_into(t, nullptr, t->rows, sp_bkeys, sp_bkeep, SP_SEED, sp_parts, first_level, true, &sp_stats[2]); };
+    while (true) {
+      TableRef b(children[1]->next());
+      if (!b.t) break;
+      if (sp_active) { split(b.t); continue; }
+      bytes += table_bytes(b.t);
+      held.emplace_back();
+      held.back().hold(b.t);
+      if (bytes <= sp_target) continue;
+      sp_active = true;
+      sp_stats[0] = sp_parts;
+      sp_buckets.resize(sp_parts);
+      sp_bkeys = build_keys;
+      sp_bkeep = carried((int)b.t->cols.size(), build_keys, build_out);
+      { TableRef sel(select(b.t, sp_bkeep)); sp_build_empty = TableRef(slice_table(sel.t, 0, 0)); }
+      b.reset();
+      for (auto& h : held) {
+        TableRef t(with_retry([&] { return h.get(); }));
+        h.close();
+        split(t.t);
+      }
+      held.clear();
+    }
+    if (sp_active) return true;
+    for (auto& h : held) parts.emplace_back(with_retry([&] { return h.get(); }));
+    return false;
+  }
+  // The stream side, split by the same keys, seed and K; through the selection vector of a GpuFilterExec directly below
+  void split_stream_side() {
+    GpuFilterExec* ff = nullptr;
+    if (kind != B2_JOIN_FULL_OUTER && !condition && !getenv("B2_NO_FILTER_FUSION")) ff = dynamic_cast<GpuFilterExec*>(children[0]);
+    std::vector<int> keys, keep;   // indices into the batches pulled (the filter's input when fused)
+    auto first_level = [&](int p) -> Bucket& { return sp_buckets[p]; };
+    while (true) {
+      TableRef raw(ff ? ff->children[0]->next() : children[0]->next());
+      if (!raw.t) break;
+      if (keep.empty()) {
+        const int ncols = ff && !ff->keep.empty() ? (int)ff->keep.size() : (int)raw.t->cols.size();
+        auto raw_of = [&](int c) { return ff && !ff->keep.empty() ? ff->keep[c] : c; };
+        for (int k : stream_keys) keys.push_back(raw_of(k));
+        for (int c : carried(ncols, stream_keys, stream_out)) keep.push_back(raw_of(c));
+        TableRef sel(select(raw.t, keep));
+        sp_stream_empty = TableRef(slice_table(sel.t, 0, 0));
+      }
+      ColGuard sel(ff ? run_as(ff, [&] { return filter_row_ids(program_from(ff->program), raw.t); }) : nullptr);
+      if (ff) { ff->num_output_rows += sel.c->size; ff->num_output_batches++; }
+      split_into(raw.t, sel.c ? sel.c->data.as<int32_t>() : nullptr, sel.c ? sel.c->size : raw.t->rows, keys, keep, SP_SEED, sp_parts,
+                 first_level, false, &sp_stats[3]);
+    }
+    if (!sp_stream_empty.t && kind == B2_JOIN_FULL_OUTER) throw Error(B2_ERR_UNSUPPORTED, "empty stream side of a full outer join needs the stream schema");
+  }
+  bool useless(const Bucket& b) const {
+    if (kind == B2_JOIN_INNER || kind == B2_JOIN_LEFT_SEMI) return b.build.empty() || b.stream.empty();
+    if (kind == B2_JOIN_FULL_OUTER) return b.build.empty() && b.stream.empty();
+    return b.stream.empty();   // LEFT OUTER / ANTI: stream rows without build rows are still output
+  }
+  // GpuSubPartitionPairIterator: a bucket still over the target is split once more, with its stream pieces.  FULL OUTER
+  // coalesces a pair's stream side, so there a bucket whose stream pieces pass the target is split again as well.
+  void repartition() {
+    Bucket b = std::move(sp_buckets.front());
+    sp_buckets.pop_front();
+    sp_stats[1]++;
+    const int64_t bytes = std::max(b.build_bytes, kind == B2_JOIN_FULL_OUTER ? b.stream_bytes : 0);
+    const int k2 = (int)std::min<int64_t>(256, std::max<int64_t>(sp_parts, bytes / sp_target + 1));
+    std::vector<Bucket> sub(k2);
+    auto second_level = [&](int p) -> Bucket& { return sub[p]; };
+    std::vector<int> all_b, all_s;
+    for (int c = 0; c < (int)sp_build_empty.t->cols.size(); c++) all_b.push_back(c);
+    for (int c = 0; sp_stream_empty.t && c < (int)sp_stream_empty.t->cols.size(); c++) all_s.push_back(c);
+    for (auto& p : b.build) { TableRef t(with_retry([&] { return p.get(); })); p.close(); split_into(t.t, nullptr, t.t->rows, build_keys, all_b, SP_RESEED, k2, second_level, true, nullptr); }
+    for (auto& p : b.stream) { TableRef t(with_retry([&] { return p.get(); })); p.close(); split_into(t.t, nullptr, t.t->rows, stream_keys, all_s, SP_RESEED, k2, second_level, false, nullptr); }
+    for (int p = k2 - 1; p >= 0; p--) { sub[p].resplit = true; sp_buckets.push_front(std::move(sub[p])); }
+  }
+  Table* concat_pieces(const std::vector<SpillPiece>& ps, const Table* empty) {
+    return with_retry([&]() -> Table* {
+      if (ps.empty()) { Table* e = const_cast<Table*>(empty); e->refs.fetch_add(1); return e; }
+      std::vector<TableRef> got;
+      std::vector<const Table*> ts;
+      for (auto& p : ps) { got.emplace_back(p.get()); ts.push_back(got.back().t); }
+      if (ts.size() == 1) return got[0].release();
+      return concat_tables(ts);
+    });
+  }
+  // GpuBatchSubPartitionIterator: the next pair = adjacent useful buckets whose build pieces together stay within the target.
+  // Builds its hash table and queues its stream pieces in probe groups of at most the target (FULL OUTER: one group).
+  bool open_next_pair() {
+    if (ht) { b2_join_hash_table_close(ht); ht = 0; }
+    build_table.reset();
+    auto over = [&](const Bucket& b) {
+      return !b.resplit && (b.build_bytes > sp_target || (kind == B2_JOIN_FULL_OUTER && b.stream_bytes > sp_target));
+    };
+    while (!sp_buckets.empty()) {
+      if (useless(sp_buckets.front())) sp_buckets.pop_front();
+      else if (over(sp_buckets.front())) repartition();
+      else break;
+    }
+    if (sp_buckets.empty()) return false;
+    // FULL OUTER coalesces the pair's stream side as well, so its stream pieces count against the target too
+    const bool full = kind == B2_JOIN_FULL_OUTER;
+    std::vector<Bucket> pair;
+    int64_t bytes = sp_buckets.front().build_bytes, sbytes = sp_buckets.front().stream_bytes;
+    pair.push_back(std::move(sp_buckets.front()));
+    sp_buckets.pop_front();
+    while (!sp_buckets.empty()) {
+      const Bucket& nb = sp_buckets.front();
+      if (useless(nb)) { sp_buckets.pop_front(); continue; }
+      if (over(nb) || bytes + nb.build_bytes > sp_target || (full && sbytes + nb.stream_bytes > sp_target)) break;
+      bytes += nb.build_bytes; sbytes += nb.stream_bytes;
+      pair.push_back(std::move(sp_buckets.front()));
+      sp_buckets.pop_front();
+    }
+    std::vector<SpillPiece> bp, sps;
+    for (auto& b : pair) {
+      for (auto& p : b.build) bp.push_back(std::move(p));
+      for (auto& p : b.stream) sps.push_back(std::move(p));
+    }
+    build_table = TableRef(concat_pieces(bp, sp_build_empty.t));
+    bp.clear();
+    ht = with_retry([&] {
+      TableRef bk(select(build_table.t, build_keys));
+      b2_handle h = 0;
+      int rc = b2_join_build(to_handle(bk.t), nulls_equal, &h);
+      if (rc != B2_OK) throw Error(rc, b2_last_error());
+      return h;
+    });
+    if (kind == B2_JOIN_FULL_OUTER) { sp_probe.push_back(std::move(sps)); return true; }
+    std::vector<SpillPiece> grp;
+    int64_t gb = 0, gr = 0;
+    for (auto& p : sps) {
+      if (!grp.empty() && (gb + p.bytes > sp_target || gr + p.rows > 0x7fffffffLL)) { sp_probe.push_back(std::move(grp)); grp.clear(); gb = gr = 0; }
+      gb += p.bytes; gr += p.rows;
+      grp.push_back(std::move(p));
+    }
+    if (!grp.empty()) sp_probe.push_back(std::move(grp));
+    return true;
+  }
+  Table* sp_next() {
+    if (!sp_read) { sp_read = true; split_stream_side(); }
+    while (true) {
+      if (!todo.empty()) return drain_todo();
+      if (!sp_probe.empty()) {
+        std::vector<SpillPiece> grp = std::move(sp_probe.front());
+        sp_probe.pop_front();
+        todo.emplace_back(TableRef(concat_pieces(grp, sp_stream_empty.t)), 0);
+        continue;
+      }
+      if (!open_next_pair()) return nullptr;
+    }
+  }
 };
 
 DevBuf sort_order(const Table* t, const b2_order_by_arg* keys, int nkeys);
@@ -704,29 +949,13 @@ struct GpuOutOfCoreSortExec : GpuExec {
   std::vector<b2_order_by_arg> order;        // the sort keys
   std::vector<b2_order_by_arg> merge_keys;   // the sort keys, then the ordinal
   int64_t target = 0;
-  struct Piece {
-    b2_handle sp = 0;
-    int64_t rows = 0, bytes = 0;
-    std::vector<int64_t> chars;    // per column: string bytes
-    std::vector<char> nullable;    // per column: carries validity
+  struct Piece : SpillPiece {
     // pending pieces: their first row, kept on the device outside the spill store (one row per piece, and there are at most
     // about 8 pieces per target_bytes of input) so that ordering the pieces never brings a spilled piece back
     TableRef head;
     Piece() {}
-    Piece(const Piece&) = delete;
-    Piece(Piece&& o) noexcept : sp(o.sp), rows(o.rows), bytes(o.bytes), chars(std::move(o.chars)), nullable(std::move(o.nullable)), head(std::move(o.head)) { o.sp = 0; }
-    Piece& operator=(Piece&& o) noexcept {
-      if (this != &o) { close(); sp = o.sp; o.sp = 0; rows = o.rows; bytes = o.bytes; chars = std::move(o.chars); nullable = std::move(o.nullable); head = std::move(o.head); }
-      return *this;
-    }
-    ~Piece() { close(); }
-    void close() { if (sp) b2_spillable_close(sp); sp = 0; }
-    Table* get() const {
-      b2_handle h = 0;
-      int rc = b2_spillable_get(sp, &h);
-      if (rc != B2_OK) throw Error(rc, b2_last_error());
-      return from_handle_owned(h);
-    }
+    Piece(Piece&&) noexcept = default;
+    Piece& operator=(Piece&&) noexcept = default;
   };
   std::vector<Piece> pending;
   std::deque<Piece> final_q;
@@ -762,11 +991,8 @@ struct GpuOutOfCoreSortExec : GpuExec {
       const int64_t e = lo;
       TableRef piece(slice_table(t, s, e));
       Piece p;
-      p.rows = e - s; p.bytes = table_bytes(piece.t);
-      for (const Column* c : piece.t->cols) { p.chars.push_back(c->dtype == B2_STRING ? c->chars_bytes : 0); p.nullable.push_back(c->nullable()); }
       if (with_heads) p.head = TableRef(slice_table(t, s, s + 1));
-      int rc = b2_spillable_create(to_handle(piece.t), &p.sp);
-      if (rc != B2_OK) throw Error(rc, b2_last_error());
+      p.hold(piece.t);
       out.push_back(std::move(p));
       s = e;
     }
@@ -1182,6 +1408,23 @@ int b2_exec_join_set_condition(b2_handle join, b2_handle condition_program) {
   auto* j = dynamic_cast<GpuShuffledHashJoinExec*>(exec_from(join));
   B2_CHECK(j, "not a hash join node");
   j->condition = condition_program;
+  B2_CATCH
+}
+int b2_exec_join_set_sub_partitioning(b2_handle join, int64_t target_bytes, int32_t num_partitions) {
+  B2_TRY
+  auto* j = dynamic_cast<GpuShuffledHashJoinExec*>(exec_from(join));
+  B2_CHECK(j, "not a hash join node");
+  B2_CHECK(num_partitions >= 2 && num_partitions <= 256, "sub-partitioning: 2 to 256 partitions");
+  B2_CHECK(!j->built, "sub-partitioning must be set before the join runs");
+  j->sp_target = std::max<int64_t>(target_bytes, 16 << 10);   // at least 16 KiB, like the sort's target
+  j->sp_parts = num_partitions;
+  B2_CATCH
+}
+int b2_exec_join_sub_partition_stats(b2_handle join, int64_t* out4) {
+  B2_TRY
+  auto* j = dynamic_cast<GpuShuffledHashJoinExec*>(exec_from(join));
+  B2_CHECK(j, "not a hash join node");
+  for (int i = 0; i < 4; i++) out4[i] = j->sp_stats[i];
   B2_CATCH
 }
 int b2_exec_broadcast_exchange(b2_handle child, b2_handle comm, int32_t rank, int32_t world, b2_handle* out) {

@@ -34,9 +34,11 @@ __global__ void __launch_bounds__(PT_NT) part_tile_hist_kernel(const Pid pids, i
 // writes one aligned vector.  Only the elements whose aligned destination vector crosses the run's ends (< 2V per run)
 // leave one by one.  (The first version stored aligned STAGE vectors and fell back to per-element loops for whole
 // misaligned runs: the profiler counted about twice the ideal store sectors and DRAM writes.)
-template <typename T, int TILE>
-__device__ __forceinline__ void ps_store(T* __restrict__ out, const T* stage, int tile_n, const uint8_t* s_owner, const int32_t* s_start,
-                                         const int32_t* s_gbase) {
+// `out_of(p)` is the array partition p's run goes to: one array for every partition (ps_store), or one per partition
+// (hash.cu's split into owned tables); each must be 16-byte aligned.
+template <typename T, int TILE, typename OutOf>
+__device__ __forceinline__ void ps_store_to(const OutOf& out_of, const T* stage, int tile_n, const uint8_t* s_owner, const int32_t* s_start,
+                                            const int32_t* s_gbase) {
   constexpr int V = sizeof(T) >= 16 ? 1 : 16 / (int)sizeof(T);
   // fixed trip count, fully unrolled: the iterations are independent and their shared-memory loads and global stores overlap.
   // (With the runtime bound `k0 < tile_n` the compiler unrolled this loop in one build and not in the next, and the kernel's
@@ -46,7 +48,7 @@ __device__ __forceinline__ void ps_store(T* __restrict__ out, const T* stage, in
   for (int it = 0; it < ITERS; it++) {
     const int k0 = (it * PT_NT + (int)threadIdx.x) * V;
     if (k0 >= tile_n) continue;
-    if (V == 1) { const int p = s_owner[k0]; __stcs(&out[(int64_t)s_gbase[p] + (k0 - s_start[p])], stage[k0]); continue; }
+    if (V == 1) { const int p = s_owner[k0]; __stcs(&out_of(p)[(int64_t)s_gbase[p] + (k0 - s_start[p])], stage[k0]); continue; }
     {
       const int p = s_owner[k0];
       const int64_t c = (int64_t)s_gbase[p] - s_start[p];       // dest(k) = k + c inside run p
@@ -55,7 +57,7 @@ __device__ __forceinline__ void ps_store(T* __restrict__ out, const T* stage, in
         // whole sectors, never touched again: streaming store.  The boundary elements below keep the default policy: their
         // sector is completed by the neighbouring tile's run, and the kernel's DRAM writes depend on those half-written
         // sectors still being in L2 when the other half arrives
-        __stcs(reinterpret_cast<uint4*>(out + (kk + c)), pack16<T>(stage + kk));
+        __stcs(reinterpret_cast<uint4*>(out_of(p) + (kk + c)), pack16<T>(stage + kk));
       }
     }
 #pragma unroll
@@ -65,10 +67,20 @@ __device__ __forceinline__ void ps_store(T* __restrict__ out, const T* stage, in
       const int q = s_owner[e];
       const int64_t c = (int64_t)s_gbase[q] - s_start[q];
       const int kk = e - (int)((e + c) % V);
-      if (!(kk >= s_start[q] && kk + V <= s_start[q + 1])) out[e + c] = stage[e];
+      if (!(kk >= s_start[q] && kk + V <= s_start[q + 1])) out_of(q)[e + c] = stage[e];
     }
   }
   __syncthreads();
+}
+template <typename T>
+struct SameOut {
+  T* __restrict__ p;
+  __device__ __forceinline__ T* operator()(int) const { return p; }
+};
+template <typename T, int TILE>
+__device__ __forceinline__ void ps_store(T* __restrict__ out, const T* stage, int tile_n, const uint8_t* s_owner, const int32_t* s_start,
+                                         const int32_t* s_gbase) {
+  ps_store_to<T, TILE>(SameOut<T>{out}, stage, tile_n, s_owner, s_start, s_gbase);
 }
 #endif
 

@@ -48,10 +48,19 @@ class GpuExec:
         return out[0], out[1]
 
 
-def _new(fn, *args, keep=()):
+class HashJoinExec(GpuExec):
+    @property
+    def sub_partition_stats(self):
+        """GpuSubPartitionHashJoin: first-level buckets (0 = not sub-partitioned), buckets repartitioned, bytes split per side"""
+        out = (ctypes.c_int64 * 4)()
+        check(lib.b2_exec_join_sub_partition_stats(self.h, out))
+        return {"buckets": out[0], "repartitioned": out[1], "build_bytes": out[2], "stream_bytes": out[3]}
+
+
+def _new(fn, *args, keep=(), cls=GpuExec):
     out = ctypes.c_int64()
     check(fn(*args, ctypes.byref(out)))
-    return GpuExec(out.value, keep)
+    return cls(out.value, keep)
 
 
 def GpuBatchSource(tables=()):
@@ -140,14 +149,19 @@ def GpuHashAggregateExec(child, grouping, aggregates, pre_project=None, conditio
                 m._agg_specs(aggregates), len(aggregates), keep=[prog, child])
 
 
-def GpuShuffledHashJoinExec(stream_keys, build_keys, join_type, stream, build, nulls_equal=False, stream_out=None, build_out=None, condition=None):
+def GpuShuffledHashJoinExec(stream_keys, build_keys, join_type, stream, build, nulls_equal=False, stream_out=None, build_out=None, condition=None,
+                            target_bytes=None, num_sub_partitions=16):
     """stream_out / build_out: columns a pruning GpuProjectExec above the join keeps (fused into the gathers);
-    condition: non-equi join condition (Expr / Program) bound over [stream columns ++ build columns] (mixed join)"""
+    condition: non-equi join condition (Expr / Program) bound over [stream columns ++ build columns] (mixed join);
+    target_bytes given: GpuSubPartitionHashJoin, a build side larger than target_bytes is split into num_sub_partitions
+    spillable buckets with the stream side and joined bucket by bucket (the build side need not fit on the device)"""
     e = _hash_join(stream_keys, build_keys, join_type, stream, build, nulls_equal, stream_out, build_out)
     if condition is not None:
         prog = condition if isinstance(condition, m.Program) else m.Program([condition])
         check(lib.b2_exec_join_set_condition(e.h, prog.h))
         e._keep.append(prog)
+    if target_bytes is not None:
+        check(lib.b2_exec_join_set_sub_partitioning(e.h, int(target_bytes), int(num_sub_partitions)))
     return e
 
 
@@ -155,9 +169,9 @@ def _hash_join(stream_keys, build_keys, join_type, stream, build, nulls_equal, s
     if stream_out is not None or build_out is not None:
         so, bo = list(stream_out or []), list(build_out or [])
         return _new(lib.b2_exec_shuffled_hash_join_select, stream.h, build.h, m._i32s(stream_keys), m._i32s(build_keys), len(stream_keys), join_type,
-                    int(nulls_equal), m._i32s(so), len(so), m._i32s(bo), len(bo), keep=[stream, build])
+                    int(nulls_equal), m._i32s(so), len(so), m._i32s(bo), len(bo), keep=[stream, build], cls=HashJoinExec)
     return _new(lib.b2_exec_shuffled_hash_join, stream.h, build.h, m._i32s(stream_keys), m._i32s(build_keys), len(stream_keys), join_type,
-                int(nulls_equal), keep=[stream, build])
+                int(nulls_equal), keep=[stream, build], cls=HashJoinExec)
 
 
 def GpuSortExec(sort_order, child, global_sort=True, target_bytes=None):
