@@ -184,6 +184,9 @@ int b2_expr_close(b2_handle expr);
 /* compile N output expressions against an input schema into one program */
 int b2_program_compile(const b2_handle* exprs, int32_t nexprs, b2_handle* out);
 int b2_program_close(b2_handle program);
+/* what a compiled program looks like to the kernels: instructions, registers, register bytes per row and rows per tile
+ * (tile_rows / 256 rows per thread; the filter's TMA-staged and the group-by's fused kernels pick their own tile) */
+int b2_program_info(b2_handle program, int32_t* ninstr, int32_t* nregs, int32_t* bytes_per_row, int32_t* tile_rows);
 /* GpuProjectExec.project: table -> table of nexprs columns, one launch */
 int b2_project(b2_handle program, b2_handle table, b2_handle* out_table);
 

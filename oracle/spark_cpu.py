@@ -445,6 +445,8 @@ def _cast(a, to):
         v = np.array([float(int(x)) for x in a.values], dtype=np.float64) / float(10 ** a.typ[2])
         return OCol(v.astype(_NP[tdt]), a.valid, (tdt, 0, 0))
     x = a.values
+    if fdt == DATE32 or tdt == DATE32 or fdt == TIMESTAMP_US or tdt == TIMESTAMP_US:
+        return _cast_datetime(a, tdt)
     if tdt == BOOL8:
         return OCol((x != 0).astype(np.int8), a.valid, (BOOL8, 0, 0))
     if fdt in (FLOAT32, FLOAT64) and tdt not in (FLOAT32, FLOAT64):
@@ -466,6 +468,32 @@ def _cast(a, to):
         return OCol(out.astype(_NP[tdt]), a.valid, (tdt, 0, 0))
     with np.errstate(all="ignore"):
         return OCol(x.astype(_NP[tdt]), a.valid, (tdt, 0, 0))
+
+
+_MICROS = 1_000_000
+
+
+def _cast_datetime(a, tdt):
+    """GpuCast.scala:314-339, 370-375, 522-537: a date is never a number; a timestamp counts microseconds, a number cast to or
+    from one counts seconds.  DATE <-> TIMESTAMP needs a time zone and is not restated."""
+    fdt, x, n = a.typ[0], a.values, len(a)
+    if fdt == DATE32 and tdt in (BOOL8, INT8, INT16, INT32, INT64, FLOAT32, FLOAT64):
+        return OCol(np.zeros(n, dtype=_NP[tdt]), np.zeros(n, bool), (tdt, 0, 0))   # always NULL
+    if fdt == TIMESTAMP_US:
+        if tdt == BOOL8:
+            return OCol((x != 0).astype(np.int8), a.valid, (BOOL8, 0, 0))
+        if tdt in (FLOAT32, FLOAT64):   # microseconds / 10^6 in double, then rounded to the target
+            return OCol((x.astype(np.float64) / float(_MICROS)).astype(_NP[tdt]), a.valid, (tdt, 0, 0))
+        if tdt in (INT8, INT16, INT32, INT64):   # floorDiv to seconds, then narrowed (wraps)
+            return OCol((x.astype(np.int64) // _MICROS).astype(_NP[tdt]), a.valid, (tdt, 0, 0))
+    if tdt == TIMESTAMP_US:
+        if fdt in (BOOL8, INT8, INT16, INT32):   # false/true -> 0/1 microseconds; byte, short, int are seconds
+            return OCol(x.astype(np.int64) * (1 if fdt == BOOL8 else _MICROS), a.valid, (tdt, 0, 0))
+        if fdt == INT64:   # castLongToTimestamp: seconds, saturating
+            hi = (2**63 - 1) // _MICROS
+            out = np.array([(2**63 - 1) if v > hi else (-2**63 if v < -hi else v * _MICROS) for v in (int(t) for t in x)], dtype=np.int64)
+            return OCol(out, a.valid, (tdt, 0, 0))
+    raise NotImplementedError("cast %d -> %d" % (fdt, tdt))
 
 
 # ------------------------------------------------------------------------------------------------

@@ -377,6 +377,12 @@ class Program:
         check(lib.b2_program_compile(arr, len(self.exprs), ctypes.byref(out)))
         self.h = ctypes.c_int64(out.value)
 
+    def info(self):
+        """-> {ninstr, nregs, bytes_per_row, tile_rows}: the compiled program's geometry"""
+        v = [ctypes.c_int32() for _ in range(4)]
+        check(lib.b2_program_info(self.h, *[ctypes.byref(x) for x in v]))
+        return dict(zip(("ninstr", "nregs", "bytes_per_row", "tile_rows"), (x.value for x in v)))
+
     def __del__(self):
         if getattr(self, "h", None) is not None and self.h.value:
             lib.b2_program_close(self.h)

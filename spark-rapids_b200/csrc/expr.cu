@@ -164,11 +164,14 @@ struct Compiler {
   static bool retype_literal(Val& v, int to_mt) {
     if (v.o.kind != OK_LIT) return false;
     if (v.mt == MT_F32 || v.mt == MT_F64 || to_mt == MT_F32 || to_mt == MT_F64) {
+      const bool from_int = v.mt != MT_F32 && v.mt != MT_F64;
       double d;
       if (v.mt == MT_F32) { float f; memcpy(&f, &v.o.lo, 4); d = f; }
       else if (v.mt == MT_F64) memcpy(&d, &v.o.lo, 8);
       else d = (double)(int64_t)v.o.lo;
-      if (to_mt == MT_F32) { float f = (float)d; v.o.lo = 0; memcpy(&v.o.lo, &f, 4); v.o.hi = 0; }
+      // an integer goes to float in one rounding, as the column path's cvt.rn.f32.s64 does: through double it would be
+      // rounded twice (2^54 + 2^30 + 1 would become 2^54 instead of 2^54 + 2^31)
+      if (to_mt == MT_F32) { float f = from_int ? (float)(int64_t)v.o.lo : (float)d; v.o.lo = 0; memcpy(&v.o.lo, &f, 4); v.o.hi = 0; }
       else if (to_mt == MT_F64) { memcpy(&v.o.lo, &d, 8); v.o.hi = 0; }
       else return false;
     } else {
@@ -405,7 +408,6 @@ struct Compiler {
     if (a.o.kind == OK_LIT) a = emit(V_MOV, MT_I128, MT_I128, MT_I128, a.nullable, 0, &a, nullptr, nullptr, a.dtype, 38, a.scale);
     if (b.o.kind == OK_LIT) b = emit(V_MOV, MT_I128, MT_I128, MT_I128, b.nullable, 0, &b, nullptr, nullptr, b.dtype, 38, b.scale);
     Val h = a_low ? b : a, l = a_low ? a : b;
-    auto pin = [&](const Val& v, bool on) { if (v.o.kind == OK_REG) reg_pinned[v.o.idx] = on; };
     const int D = B2_DECIMAL128, I = MT_I128;
     pin(h, true);
     Val hq = emit(V_RESCALE_DOWN, I, I, I, h.nullable, ds, &h, nullptr, nullptr, D, 38, l.scale);
@@ -486,8 +488,88 @@ struct Compiler {
     bool commut = e->op == B2_OP_ADD || e->op == B2_OP_MUL;
     if (a.o.kind == OK_LIT && commut) std::swap(a, b);
     if (a.o.kind == OK_LIT) a = emit(V_MOV, a.mt, a.mt, a.mt, a.nullable, 0, &a, nullptr, nullptr, a.dtype, a.precision, a.scale);
-    bool div_like = e->op == B2_OP_DIV || e->op == B2_OP_MOD || e->op == B2_OP_PMOD;
+    // x / 0 and x % 0 are NULL; a non-zero literal divisor cannot make one
+    bool div_like = (e->op == B2_OP_DIV || e->op == B2_OP_MOD || e->op == B2_OP_PMOD) && !nonzero_literal(b);
     return emit(vop, a.mt, a.mt, a.mt, a.nullable || b.nullable || div_like, 0, &a, &b, nullptr, a.dtype, 0, 0);
+  }
+
+  static bool nonzero_literal(const Val& v) {
+    if (v.o.kind != OK_LIT || v.o.lit_null) return false;
+    if (v.mt == MT_F32) { float f; memcpy(&f, &v.o.lo, 4); return f != 0; }
+    if (v.mt == MT_F64) { double d; memcpy(&d, &v.o.lo, 8); return d != 0; }
+    return v.o.lo != 0 || v.o.hi != 0;
+  }
+  Val int_lit(int64_t x, int mt, int dtype) {
+    Val v; v.o = lit(x, x < 0 ? -1 : 0, false); v.mt = mt; v.dtype = dtype; v.precision = 0; v.scale = 0; v.nullable = false;
+    return v;
+  }
+  void pin(const Val& v, bool on) { if (v.o.kind == OK_REG) reg_pinned[v.o.idx] = on; }
+
+  // floorDiv(x, d) for INT64 x and a positive d: q = x / d, then IF(x % d < 0, q - 1, q)
+  Val floor_div(Val x, int64_t d) {
+    const int I = MT_I64;
+    const Val dv = int_lit(d, I, B2_INT64), zero = int_lit(0, I, B2_INT64), one = int_lit(1, I, B2_INT64);
+    pin(x, true);
+    Val q = emit(V_DIV, I, I, I, x.nullable, 0, &x, &dv, nullptr, B2_INT64, 0, 0);
+    pin(x, false);
+    pin(q, true);
+    Val r = emit(V_MOD, I, I, I, x.nullable, 0, &x, &dv, nullptr, B2_INT64, 0, 0);
+    Val neg = emit(V_LT, I, MT_I8, MT_I8, r.nullable, 0, &r, &zero, nullptr, B2_BOOL8, 0, 0);
+    Val qm = emit(V_SUB, I, I, I, q.nullable, 0, &q, &one, nullptr, B2_INT64, 0, 0);
+    pin(q, false);
+    return emit(V_IF, I, I, I, q.nullable, 0, &neg, &qm, &q, B2_INT64, 0, 0);
+  }
+
+  // GpuCast.castLongToTimestamp: seconds -> microseconds, saturating at the INT64 range
+  Val seconds_to_micros(Val x) {
+    const int I = MT_I64;
+    const int64_t max_s = INT64_MAX / 1000000;
+    const Val us = int_lit(1000000, I, B2_INT64), hi = int_lit(max_s, I, B2_INT64), lo = int_lit(-max_s, I, B2_INT64);
+    const Val sat_hi = int_lit(INT64_MAX, I, B2_TIMESTAMP_US), sat_lo = int_lit(INT64_MIN, I, B2_TIMESTAMP_US);
+    pin(x, true);
+    Val m = emit(V_MUL, I, I, I, x.nullable, 0, &x, &us, nullptr, B2_TIMESTAMP_US, 0, 0);
+    Val over = emit(V_GT, I, MT_I8, MT_I8, x.nullable, 0, &x, &hi, nullptr, B2_BOOL8, 0, 0);
+    Val r1 = emit(V_IF, I, I, I, m.nullable, 0, &over, &sat_hi, &m, B2_TIMESTAMP_US, 0, 0);
+    pin(x, false);
+    Val under = emit(V_LT, I, MT_I8, MT_I8, x.nullable, 0, &x, &lo, nullptr, B2_BOOL8, 0, 0);
+    return emit(V_IF, I, I, I, r1.nullable, 0, &under, &sat_lo, &r1, B2_TIMESTAMP_US, 0, 0);
+  }
+
+  // GpuCast.doCast for DATE32 and TIMESTAMP_US (GpuCast.scala:314-339, 370-375, 522-537).  The ABI carries no time zone, so
+  // DATE <-> TIMESTAMP is refused, as are the casts Spark has no rule for (integer -> DATE, float -> TIMESTAMP).
+  Val compile_datetime_cast(Val a, int to) {
+    const int from = a.dtype;
+    if (from == B2_DATE32) {
+      if (to == B2_TIMESTAMP_US) throw Error(B2_ERR_UNSUPPORTED, "DATE -> TIMESTAMP needs a time zone");
+      // date -> boolean or any number is always NULL
+      Val v; v.o = lit(0, 0, true); v.mt = mt_of(to); v.dtype = to; v.precision = 0; v.scale = 0; v.nullable = true;
+      return v;
+    }
+    if (to == B2_DATE32) throw Error(B2_ERR_UNSUPPORTED, from == B2_TIMESTAMP_US ? "TIMESTAMP -> DATE needs a time zone" : "cast to DATE from this type");
+    if (from == B2_TIMESTAMP_US) {
+      if (to == B2_BOOL8) return a;   // x != 0, below
+      if (to == B2_FLOAT64 || to == B2_FLOAT32) {   // microseconds / 10^6 in double, then rounded to the target
+        Val d = emit(V_CAST, MT_I64, MT_F64, MT_F64, a.nullable, 0, &a, nullptr, nullptr, B2_FLOAT64, 0, 0);
+        double us = 1e6;
+        Val dv; dv.o = lit(0, 0, false); memcpy(&dv.o.lo, &us, 8); dv.mt = MT_F64; dv.dtype = B2_FLOAT64; dv.precision = 0; dv.scale = 0; dv.nullable = false;
+        Val r = emit(V_DIV, MT_F64, MT_F64, MT_F64, d.nullable, 0, &d, &dv, nullptr, B2_FLOAT64, 0, 0);
+        if (to == B2_FLOAT32) r = emit(V_CAST, MT_F64, MT_F32, MT_F32, r.nullable, 0, &r, nullptr, nullptr, B2_FLOAT32, 0, 0);
+        return r;
+      }
+      // seconds = floorDiv(microseconds, 10^6), then narrowed like any integer
+      Val s = floor_div(a, 1000000);
+      s = widen_int(s, mt_of(to));
+      s.dtype = to;
+      return s;
+    }
+    // to == B2_TIMESTAMP_US
+    if (from == B2_FLOAT32 || from == B2_FLOAT64) throw Error(B2_ERR_UNSUPPORTED, "float -> TIMESTAMP is not supported");
+    if (from == B2_BOOL8) { Val r = widen_int(a, MT_I64); r.dtype = to; return r; }   // false/true -> 0/1 microseconds
+    if (from == B2_INT64) return seconds_to_micros(a);
+    // byte, short, int seconds cannot overflow in microseconds
+    Val w = widen_int(a, MT_I64);
+    const Val us = int_lit(1000000, MT_I64, B2_INT64);
+    return emit(V_MUL, MT_I64, MT_I64, MT_I64, w.nullable, 0, &w, &us, nullptr, B2_TIMESTAMP_US, 0, 0);
   }
 
   Val compile_cast(Expr* e) {  // GpuCast.scala:295 doCast (numeric subset)
@@ -506,6 +588,10 @@ struct Compiler {
         return r;
       }
       throw Error(B2_ERR_UNSUPPORTED, "decimal -> integral cast is not supported yet");
+    }
+    if (a.dtype == B2_DATE32 || a.dtype == B2_TIMESTAMP_US || to == B2_DATE32 || to == B2_TIMESTAMP_US) {
+      a = compile_datetime_cast(a, to);
+      if (a.dtype == to) return a;
     }
     int smt = a.mt, dmt = mt_of(to);
     if (to == B2_BOOL8) {  // x != 0
@@ -697,6 +783,12 @@ int b2_expr_type(b2_handle h, int32_t* dtype, int32_t* precision, int32_t* scale
 int b2_program_compile(const b2_handle* exprs, int32_t nexprs, b2_handle* out) {
   B2_TRY
   *out = to_handle(compile_program(exprs, nexprs));
+  B2_CATCH
+}
+int b2_program_info(b2_handle program, int32_t* ninstr, int32_t* nregs, int32_t* bytes_per_row, int32_t* tile_rows) {
+  B2_TRY
+  const Program* p = program_from(program);
+  *ninstr = p->hdr.ninstr; *nregs = p->hdr.nregs; *bytes_per_row = p->hdr.bytes_per_row; *tile_rows = p->hdr.tile_rows;
   B2_CATCH
 }
 int b2_program_close(b2_handle h) {
