@@ -429,6 +429,19 @@ int b2_exec_expand(b2_handle child, const b2_handle* projection_programs, int32_
 typedef enum { B2_AGG_MODE_PARTIAL = 0, B2_AGG_MODE_FINAL = 1, B2_AGG_MODE_COMPLETE = 2 } b2_agg_mode;
 int b2_exec_hash_aggregate(b2_handle child, b2_handle program, int32_t has_predicate, int32_t mode,
                            const int32_t* keys, int32_t nkeys, const b2_agg_spec* aggs, int32_t naggs, b2_handle* out);
+/* GpuMergeAggregateIterator repartitioning (GpuAggregateExec.scala:150-307, 863-1103), for partial results larger than the
+ * device.  Every piece (a first-pass partial; in FINAL mode an input batch) is held in the spill store.  When the held bytes
+ * (table_bytes) pass target_bytes they are merged into one; a result of at most target_bytes / 2 stays the only held piece,
+ * a larger one is split by murmur3 seed 107 of the keys into num_buckets (2..256; Spark default 16) spillable buckets, and
+ * so is every later piece.  A bucket still over the target is split again with seed 107 + 7 * depth, down to depth 10, and
+ * then merged as it is; otherwise adjacent buckets are taken while they stay within the target and merged into one output
+ * batch.  Memory: at most target_bytes of partials per merge (except a bucket at depth 10), plus that merge's workspace;
+ * the rows of a single key must fit on the device.  Output rows and batches differ from the single merge's in order only.
+ * Without this call, on a keyless aggregate (accepted, no effect), or when the held pieces never pass the target, the node
+ * is unchanged.  B2_ERR_INVALID: target_bytes <= 0, num_buckets outside 2..256, not an aggregate, or already running. */
+int b2_exec_aggregate_set_repartitioning(b2_handle agg, int64_t target_bytes, int32_t num_buckets);
+/* out4: first-level buckets (0 = never bucketed), buckets split again, bytes split over all levels, deepest level reached */
+int b2_exec_aggregate_repartition_stats(b2_handle agg, int64_t* out4);
 /* GpuShuffledHashJoinExec (GpuShuffledHashJoinExec.scala:228-385): output = stream columns ++ build columns */
 int b2_exec_shuffled_hash_join(b2_handle stream_child, b2_handle build_child, const int32_t* stream_keys,
                                const int32_t* build_keys, int32_t nkeys, int32_t kind, int32_t nulls_equal, b2_handle* out);

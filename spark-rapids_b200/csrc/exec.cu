@@ -102,6 +102,36 @@ struct SpillPiece {
   }
 };
 
+static std::vector<TableRef> owned(std::vector<Table*>&& ts) {
+  std::vector<TableRef> out;
+  for (Table* t : ts) out.emplace_back(t);
+  return out;
+}
+// GpuBatchSubPartitioner, shared by the join's sub-partitioning and the aggregate's repartitioning: the rows of t (or the n rows
+// d_sel names), columns `keep`, split by pmod(murmur3(keys, seed), nparts) into spill pieces; put(p, piece) for every non-empty p
+template <typename Put>
+static void split_pieces(const Table* t, const int32_t* d_sel, int64_t n, const std::vector<int>& keys, const std::vector<int>& keep, int seed,
+                         int nparts, Put&& put) {
+  std::vector<TableRef> parts = owned(with_retry([&] { return hash_split_table(t, d_sel, n, keys.data(), (int)keys.size(), (uint32_t)seed, nparts, keep); }));
+  for (int p = 0; p < nparts; p++) {
+    if (!parts[p].t) continue;
+    SpillPiece s;
+    s.hold(parts[p].t);
+    put(p, std::move(s));
+  }
+}
+// the pieces brought back and concatenated (a new reference to `empty` when there are none)
+static Table* concat_pieces(const std::vector<SpillPiece>& ps, const Table* empty) {
+  return with_retry([&]() -> Table* {
+    if (ps.empty()) { Table* e = const_cast<Table*>(empty); e->refs.fetch_add(1); return e; }
+    std::vector<TableRef> got;
+    std::vector<const Table*> ts;
+    for (auto& p : ps) { got.emplace_back(p.get()); ts.push_back(got.back().t); }
+    if (ts.size() == 1) return got[0].release();
+    return concat_tables(ts);
+  });
+}
+
 struct GpuExec {
   std::atomic<int> refs{1};
   std::vector<GpuExec*> children;
@@ -361,7 +391,9 @@ struct GpuHashAggregateExec : GpuExec {
     for (Column* c : cols) col_incref(c);
     return new_table(std::move(cols));
   }
-  Table* merge(const Table* t) {  // keys are the leading columns, then the aggregates, then the counts
+  // keys are the leading columns, then the aggregates, then the counts; keep_counts: an intermediate merge, whose result is
+  // merged again, keeps the counts in every mode
+  Table* merge(const Table* t, bool keep_counts = false) {
     const int nk = (int)keys.size(), na = (int)aggs.size(), nc = (int)counted.size();
     std::vector<b2_agg_spec> m = merge_specs(update_specs(), nk);
     // flag the partial decimal sums that overflowed; only when there are any does the merge carry them (MAX of the flags)
@@ -400,7 +432,7 @@ struct GpuHashAggregateExec : GpuExec {
              r.t->cols[nk + na + nc + q]->data.as<int8_t>(), r.t->rows);
       s->null_count = -1;
     }
-    std::vector<Column*> out(r.t->cols.begin(), r.t->cols.begin() + nk + na + (mode == B2_AGG_MODE_PARTIAL ? nc : 0));
+    std::vector<Column*> out(r.t->cols.begin(), r.t->cols.begin() + nk + na + (mode == B2_AGG_MODE_PARTIAL || keep_counts ? nc : 0));
     for (Column* c : out) col_incref(c);
     return new_table(std::move(out));
   }
@@ -419,6 +451,7 @@ struct GpuHashAggregateExec : GpuExec {
     }
   }
   Table* do_next() override {
+    if (rp_target > 0 && !keys.empty()) return rp_next();
     if (done) return nullptr;
     done = true;
     std::vector<TableRef> partials;
@@ -428,6 +461,9 @@ struct GpuHashAggregateExec : GpuExec {
       if (mode == B2_AGG_MODE_FINAL) partials.emplace_back(in.release());   // inputs already are aggregation buffers
       else first_pass(in.t, partials, 0);
     }
+    return merge_all(partials);
+  }
+  Table* merge_all(std::vector<TableRef>& partials) {
     if (partials.empty()) {
       // a keyless aggregate over no batches still emits its initial-value row (GpuAggregateExec.scala:1107-1126)
       if (!keys.empty() || mode == B2_AGG_MODE_FINAL) return nullptr;
@@ -438,6 +474,128 @@ struct GpuHashAggregateExec : GpuExec {
     for (auto& p : partials) ts.push_back(p.t);
     TableRef cat(concat_tables(ts));
     return merge(cat.t);
+  }
+
+  // ---- repartitioning (GpuMergeAggregateIterator, AggregateUtils.iterateAndRepartition: GpuAggregateExec.scala:150-307, 863-1103)
+  // Seeds 107 + 7 * depth, not the exchange's 42: a FINAL aggregate's input arrives split by pmod(murmur3_42(keys), world), and
+  // buckets by the same hash would leave most of them empty on each rank.  Equal keys always meet in one bucket: murmur_col
+  // hashes every NaN payload alike, -0.0 as 0.0 and NULL as the seed.
+  static constexpr int RP_SEED = 107, RP_SEED_STEP = 7, RP_MAX_DEPTH = 10;
+  int64_t rp_target = 0;   // 0: off
+  int rp_parts = 16;
+  int64_t rp_stats[4] = {0, 0, 0, 0};   // first-level buckets, buckets split again, bytes split, deepest level
+  struct AggBucket {
+    std::vector<SpillPiece> pieces;
+    int64_t bytes = 0;
+    int depth = 0;
+  };
+  std::deque<AggBucket> rp_buckets;
+
+  // pieces are partial buffers (PARTIAL / COMPLETE) or input buffers (FINAL): the keys lead, every column is carried
+  template <typename BucketOf>
+  void rp_split(const Table* t, int depth, BucketOf&& bucket_of) {
+    std::vector<int> kc, all;
+    for (int k = 0; k < (int)keys.size(); k++) kc.push_back(k);
+    for (int c = 0; c < (int)t->cols.size(); c++) all.push_back(c);
+    split_pieces(t, nullptr, t->rows, kc, all, RP_SEED + RP_SEED_STEP * depth, rp_parts, [&](int p, SpillPiece&& s) {
+      AggBucket& b = bucket_of(p);
+      b.bytes += s.bytes;
+      rp_stats[2] += s.bytes;
+      b.pieces.push_back(std::move(s));
+    });
+  }
+  // Pull phase: every piece (a first-pass partial; in FINAL mode an input batch) waits in the spill store.  When the held bytes
+  // pass the target they are merged into one, counts kept; a result of at most half the target stays the only held piece, a
+  // larger one is split into the first-level buckets, and so is every later piece.  True: bucketed.  False: the held pieces
+  // never passed the target and are in `partials`.
+  bool rp_pull(std::vector<TableRef>& partials) {
+    std::vector<SpillPiece> held;
+    int64_t bytes = 0;
+    bool bucketed = false;
+    auto first_level = [&](int p) -> AggBucket& { return rp_buckets[p]; };
+    auto take = [&](TableRef piece) {
+      if (bucketed) { rp_split(piece.t, 0, first_level); return; }
+      held.emplace_back();
+      held.back().hold(piece.t);
+      bytes += held.back().bytes;
+      piece.reset();
+      if (bytes <= rp_target) return;
+      const bool unique = held.size() == 1 && mode != B2_AGG_MODE_FINAL;   // a single partial is key-unique already
+      TableRef cat(concat_pieces(held, nullptr));
+      held.clear();
+      TableRef merged(unique ? cat.release() : with_retry([&] { return merge(cat.t, true); }));
+      cat.reset();
+      if (table_bytes(merged.t) <= rp_target / 2) {
+        held.emplace_back();
+        held.back().hold(merged.t);
+        bytes = held.back().bytes;
+        return;
+      }
+      bucketed = true;
+      rp_stats[0] = rp_parts;
+      rp_buckets.resize(rp_parts);
+      rp_split(merged.t, 0, first_level);
+    };
+    while (true) {
+      TableRef in(children[0]->next());
+      if (!in.t) break;
+      if (mode == B2_AGG_MODE_FINAL) { take(std::move(in)); continue; }
+      std::vector<TableRef> ps;
+      first_pass(in.t, ps, 0);
+      in.reset();
+      for (auto& p : ps) take(std::move(p));
+    }
+    if (bucketed) return true;
+    for (auto& h : held) partials.emplace_back(with_retry([&] { return h.get(); }));
+    return false;
+  }
+  void rp_resplit() {
+    AggBucket b = std::move(rp_buckets.front());
+    rp_buckets.pop_front();
+    const int depth = b.depth + 1;
+    rp_stats[1]++;
+    rp_stats[3] = std::max<int64_t>(rp_stats[3], depth);
+    std::vector<AggBucket> sub(rp_parts);
+    auto next_level = [&](int p) -> AggBucket& { return sub[p]; };
+    for (auto& p : b.pieces) {
+      TableRef t(with_retry([&] { return p.get(); }));
+      p.close();
+      rp_split(t.t, depth, next_level);
+    }
+    for (int p = rp_parts - 1; p >= 0; p--) { sub[p].depth = depth; rp_buckets.push_front(std::move(sub[p])); }
+  }
+  // Finish phase, one output batch per call: a bucket over the target is split again into buckets that take its place, down to
+  // depth 10; otherwise adjacent buckets are taken while their bytes stay within the target (at least one) and merged
+  Table* rp_next() {
+    if (!done) {
+      done = true;
+      std::vector<TableRef> partials;
+      if (!rp_pull(partials)) return merge_all(partials);
+    }
+    while (!rp_buckets.empty()) {
+      const AggBucket& f = rp_buckets.front();
+      if (f.pieces.empty()) rp_buckets.pop_front();
+      else if (f.bytes > rp_target && f.depth < RP_MAX_DEPTH) rp_resplit();
+      else break;
+    }
+    if (rp_buckets.empty()) return nullptr;
+    std::vector<SpillPiece> grp;
+    int64_t bytes = 0, rows = 0;
+    while (!rp_buckets.empty()) {
+      AggBucket& b = rp_buckets.front();
+      int64_t brows = 0;
+      for (auto& p : b.pieces) brows += p.rows;
+      if (!grp.empty() && !b.pieces.empty() && (bytes + b.bytes > rp_target || rows + brows > 0x7fffffffLL)) break;
+      bytes += b.bytes;
+      rows += brows;
+      for (auto& p : b.pieces) grp.push_back(std::move(p));
+      rp_buckets.pop_front();
+    }
+    const bool unique = grp.size() == 1 && mode != B2_AGG_MODE_FINAL;   // a FINAL input batch may repeat keys
+    TableRef cat(concat_pieces(grp, nullptr));
+    grp.clear();
+    if (unique) return without_counts(cat.release());
+    return with_retry([&] { return merge(cat.t); });
   }
 };
 
@@ -707,24 +865,15 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
     for (int& c : out_cols) c = pos(c);
     return keep;
   }
-  static std::vector<TableRef> owned(std::vector<Table*>&& ts) {
-    std::vector<TableRef> out;
-    for (Table* t : ts) out.emplace_back(t);
-    return out;
-  }
   template <typename BucketOf>
   void split_into(const Table* t, const int32_t* d_sel, int64_t n, const std::vector<int>& keys, const std::vector<int>& keep, int seed, int nparts,
                   BucketOf&& bucket_of, bool build_side, int64_t* bytes_out) {
-    std::vector<TableRef> parts = owned(with_retry([&] { return hash_split_table(t, d_sel, n, keys.data(), (int)keys.size(), (uint32_t)seed, nparts, keep); }));
-    for (int p = 0; p < nparts; p++) {
-      if (!parts[p].t) continue;
+    split_pieces(t, d_sel, n, keys, keep, seed, nparts, [&](int p, SpillPiece&& s) {
       Bucket& b = bucket_of(p);
-      std::vector<SpillPiece>& dst = build_side ? b.build : b.stream;
-      dst.emplace_back();
-      dst.back().hold(parts[p].t);
-      (build_side ? b.build_bytes : b.stream_bytes) += dst.back().bytes;
-      if (bytes_out) *bytes_out += dst.back().bytes;
-    }
+      (build_side ? b.build_bytes : b.stream_bytes) += s.bytes;
+      if (bytes_out) *bytes_out += s.bytes;
+      (build_side ? b.build : b.stream).push_back(std::move(s));
+    });
   }
   // Pulls the build side into the spill store.  False: it stayed within the target and `parts` holds its batches.  True: it
   // passed the target and is split into the buckets.
@@ -804,16 +953,6 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
     for (auto& p : b.build) { TableRef t(with_retry([&] { return p.get(); })); p.close(); split_into(t.t, nullptr, t.t->rows, build_keys, all_b, SP_RESEED, k2, second_level, true, nullptr); }
     for (auto& p : b.stream) { TableRef t(with_retry([&] { return p.get(); })); p.close(); split_into(t.t, nullptr, t.t->rows, stream_keys, all_s, SP_RESEED, k2, second_level, false, nullptr); }
     for (int p = k2 - 1; p >= 0; p--) { sub[p].resplit = true; sp_buckets.push_front(std::move(sub[p])); }
-  }
-  Table* concat_pieces(const std::vector<SpillPiece>& ps, const Table* empty) {
-    return with_retry([&]() -> Table* {
-      if (ps.empty()) { Table* e = const_cast<Table*>(empty); e->refs.fetch_add(1); return e; }
-      std::vector<TableRef> got;
-      std::vector<const Table*> ts;
-      for (auto& p : ps) { got.emplace_back(p.get()); ts.push_back(got.back().t); }
-      if (ts.size() == 1) return got[0].release();
-      return concat_tables(ts);
-    });
   }
   // GpuBatchSubPartitionIterator: the next pair = adjacent useful buckets whose build pieces together stay within the target.
   // Builds its hash table and queues its stream pieces in probe groups of at most the target (FULL OUTER: one group).
@@ -1377,6 +1516,24 @@ int b2_exec_hash_aggregate(b2_handle child, b2_handle program, int32_t has_predi
   e->init_counted();
   e->add_child(exec_from(child));
   *out = to_handle(e.release());
+  B2_CATCH
+}
+int b2_exec_aggregate_set_repartitioning(b2_handle agg, int64_t target_bytes, int32_t num_buckets) {
+  B2_TRY
+  auto* a = dynamic_cast<GpuHashAggregateExec*>(exec_from(agg));
+  B2_CHECK(a, "not a hash aggregate node");
+  B2_CHECK(target_bytes > 0, "repartitioning: target_bytes must be positive");
+  B2_CHECK(num_buckets >= 2 && num_buckets <= 256, "repartitioning: 2 to 256 buckets");
+  B2_CHECK(!a->done, "repartitioning must be set before the aggregate runs");
+  a->rp_target = target_bytes;
+  a->rp_parts = num_buckets;
+  B2_CATCH
+}
+int b2_exec_aggregate_repartition_stats(b2_handle agg, int64_t* out4) {
+  B2_TRY
+  auto* a = dynamic_cast<GpuHashAggregateExec*>(exec_from(agg));
+  B2_CHECK(a, "not a hash aggregate node");
+  for (int i = 0; i < 4; i++) out4[i] = a->rp_stats[i];
   B2_CATCH
 }
 int b2_exec_shuffled_hash_join(b2_handle stream_child, b2_handle build_child, const int32_t* stream_keys, const int32_t* build_keys, int32_t nkeys,

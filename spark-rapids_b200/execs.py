@@ -132,21 +132,37 @@ def GpuExpandExec(projections, child):
     return _new(lib.b2_exec_expand, child.h, arr, len(progs), keep=progs + [child])
 
 
-def GpuHashAggregateExec(child, grouping, aggregates, pre_project=None, condition=None, mode="partial"):
+class HashAggregateExec(GpuExec):
+    @property
+    def repartition_stats(self):
+        """GpuMergeAggregateIterator: first-level buckets (0 = never bucketed), buckets split again, bytes split over all
+        levels, deepest level reached"""
+        out = (ctypes.c_int64 * 4)()
+        check(lib.b2_exec_aggregate_repartition_stats(self.h, out))
+        return {"buckets": out[0], "resplit": out[1], "bytes_split": out[2], "depth": out[3]}
+
+
+def GpuHashAggregateExec(child, grouping, aggregates, pre_project=None, condition=None, mode="partial", target_bytes=None, num_buckets=16):
     """mode 'partial'/'complete': update aggregates over `pre_project` expressions (with `condition`
     fused in as the child filter); 'final': merge aggregation buffers whose keys lead the input.
     A 'partial' output (a 'final' input) is the keys, one column per aggregate, then one INT64 count of
-    valid inputs per decimal SUM (Spark's isEmpty), so that a partial sum that overflowed stays NULL."""
+    valid inputs per decimal SUM (Spark's isEmpty), so that a partial sum that overflowed stays NULL.
+    target_bytes given: once the held partials pass target_bytes they are split into num_buckets spillable hash buckets
+    and merged bucket by bucket, one output batch per group of buckets (the partials need not fit on the device)"""
     code = {"partial": 0, "final": 1, "complete": 2}[mode]
     if mode == "final":
-        return _new(lib.b2_exec_hash_aggregate, child.h, ctypes.c_int64(0), 0, code, m._i32s(grouping), len(grouping), m._agg_specs(aggregates),
-                    len(aggregates), keep=[child])
-    if isinstance(pre_project, m.Program):    # compiled once per plan (output 0 is the fused condition when `condition` is truthy)
-        prog = pre_project
+        e = _new(lib.b2_exec_hash_aggregate, child.h, ctypes.c_int64(0), 0, code, m._i32s(grouping), len(grouping), m._agg_specs(aggregates),
+                 len(aggregates), keep=[child], cls=HashAggregateExec)
     else:
-        prog = m.Program(([condition] if condition is not None else []) + list(pre_project))
-    return _new(lib.b2_exec_hash_aggregate, child.h, prog.h, int(condition is not None), code, m._i32s(grouping), len(grouping),
-                m._agg_specs(aggregates), len(aggregates), keep=[prog, child])
+        if isinstance(pre_project, m.Program):    # compiled once per plan (output 0 is the fused condition when `condition` is truthy)
+            prog = pre_project
+        else:
+            prog = m.Program(([condition] if condition is not None else []) + list(pre_project))
+        e = _new(lib.b2_exec_hash_aggregate, child.h, prog.h, int(condition is not None), code, m._i32s(grouping), len(grouping),
+                 m._agg_specs(aggregates), len(aggregates), keep=[prog, child], cls=HashAggregateExec)
+    if target_bytes is not None:
+        check(lib.b2_exec_aggregate_set_repartitioning(e.h, int(target_bytes), int(num_buckets)))
+    return e
 
 
 def GpuShuffledHashJoinExec(stream_keys, build_keys, join_type, stream, build, nulls_equal=False, stream_out=None, build_out=None, condition=None,
