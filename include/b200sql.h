@@ -244,7 +244,11 @@ int b2_distinct_count(b2_handle table, const int32_t* key_cols, int32_t nkeys, i
 /* ---- a6/a7: hash join (GpuHashJoin.scala:256-600, 1374-1553; JoinGatherer.scala:585-599) ------- */
 typedef enum {
   B2_JOIN_INNER = 0, B2_JOIN_LEFT_OUTER = 1, B2_JOIN_LEFT_SEMI = 2, B2_JOIN_LEFT_ANTI = 3,
-  B2_JOIN_FULL_OUTER = 4
+  B2_JOIN_FULL_OUTER = 4,
+  /* every build row appears; stream columns NULL where no stream row matched.  Spark's RightOuter with BuildRight, and
+   * LeftOuter with BuildLeft with the children swapped (the caller restores the column order with a bound-reference
+   * projection) — HashOuterJoinIterator (GpuShuffledSizedHashJoinExec.scala:346-364, GpuHashJoin.scala:1807-1814) */
+  B2_JOIN_RIGHT_OUTER = 5
 } b2_join_kind;
 /* build once per build batch (the reference rebuilds per stream batch: JoinPrimitives.hashInnerJoin
  * takes both key tables each call).  nulls_equal = compareNullsEqual (GpuHashJoin.scala:602-640) */
@@ -254,7 +258,8 @@ int b2_join_hash_table_close(b2_handle ht);
  * For LEFT_OUTER unmatched rows carry INT32_MIN in the right map (OutOfBoundsPolicy.NULLIFY).
  * FULL_OUTER = the LEFT_OUTER maps followed by one row per build row that no stream row matched, in build order,
  * with INT32_MIN in the left map (Table.fullJoinGatherMaps; across stream batches the caller keeps the union of
- * matched build rows itself, as GpuHashJoin.scala's HashFullJoinIterator does). */
+ * matched build rows itself, as GpuHashJoin.scala's HashFullJoinIterator does).  RIGHT_OUTER = the INNER maps followed by
+ * (INT32_MIN, b) for every build row b no stream row matched, ascending (through a selection vector too). */
 int b2_join_probe(b2_handle ht, b2_handle probe_keys_table, int32_t kind,
                   b2_handle* out_left_map, b2_handle* out_right_map);
 /* late materialisation: `selection` = INT32 row ids (ascending) of the stream rows that take part, e.g. the rows a
@@ -269,6 +274,21 @@ int b2_join_probe_sel(b2_handle ht, b2_handle probe_keys_table, b2_handle select
  * `table`.  The left map carries ORIGINAL row ids of `table`; out_npass = rows that passed the filter. */
 int b2_join_probe_filter(b2_handle ht, b2_handle table, int32_t key_col, b2_handle predicate_program,
                          b2_handle* out_left_map, b2_handle* out_right_map, int64_t* out_npass);
+/* Matched build rows across stream batches, for outer joins that preserve the build side: a tracker is one bit per build row
+ * of ONE hash table (zeroed at creation), kept apart from the table because a cached table is shared by task threads.
+ * b2_join_probe_track = b2_join_probe_sel (kind INNER or LEFT_OUTER) that also sets the bit of every build row it finds,
+ * inside the probe kernel (HashJoinStreamSideIterator.updateTrackingMask, GpuHashJoin.scala:2164-2204; the sub-partitioned
+ * join keeps one per pair, GpuShuffledSizedHashJoinExec.scala:1760); a tracker of another table: B2_ERR_INVALID.
+ * b2_join_tracker_mark sets the bits of right_map[i] where pass[i] (BOOL8, NULL = false; pass = 0: every i) — the pairs that
+ * passed a join condition; negative entries are skipped, one >= the build row count gives B2_ERR_INVALID.  Marking is
+ * idempotent.  b2_join_tracker_unmatched: ascending INT32 ids of the build rows never marked (HashOuterJoinIterator.getFinalBatch,
+ * GpuHashJoin.scala:2288-2326). */
+int b2_join_tracker_create(b2_handle ht, b2_handle* out_tracker);
+int b2_join_tracker_close(b2_handle tracker);
+int b2_join_probe_track(b2_handle ht, b2_handle probe_keys_table, b2_handle selection, int32_t kind, b2_handle tracker,
+                        b2_handle* out_left_map, b2_handle* out_right_map);
+int b2_join_tracker_mark(b2_handle tracker, b2_handle right_map, b2_handle pass);
+int b2_join_tracker_unmatched(b2_handle tracker, b2_handle* out_ids);
 /* Table.gather(map, OutOfBoundsPolicy): out-of-range index -> null row when nullify != 0 */
 int b2_gather(b2_handle table, b2_handle int32_map, int32_t nullify_oob, b2_handle* out_table);
 
@@ -442,7 +462,10 @@ int b2_exec_hash_aggregate(b2_handle child, b2_handle program, int32_t has_predi
 int b2_exec_aggregate_set_repartitioning(b2_handle agg, int64_t target_bytes, int32_t num_buckets);
 /* out4: first-level buckets (0 = never bucketed), buckets split again, bytes split over all levels, deepest level reached */
 int b2_exec_aggregate_repartition_stats(b2_handle agg, int64_t* out4);
-/* GpuShuffledHashJoinExec (GpuShuffledHashJoinExec.scala:228-385): output = stream columns ++ build columns */
+/* GpuShuffledHashJoinExec (GpuShuffledHashJoinExec.scala:228-385): output = stream columns ++ build columns.  RIGHT_OUTER joins
+ * the stream batches one at a time, tracking the build rows found (b2_join_probe_track), and after the last one emits the
+ * unmatched build rows with NULL stream columns, in batches halved until they fit; no stream batch at all, or no build
+ * batch: B2_ERR_UNSUPPORTED.  FULL_OUTER without a condition coalesces the stream side into one batch. */
 int b2_exec_shuffled_hash_join(b2_handle stream_child, b2_handle build_child, const int32_t* stream_keys,
                                const int32_t* build_keys, int32_t nkeys, int32_t kind, int32_t nulls_equal, b2_handle* out);
 /* same with a column-pruning GpuProjectExec above the join fused into the gathers: output = stream_out ++ build_out */
@@ -452,12 +475,14 @@ int b2_exec_shuffled_hash_join_select(b2_handle stream_child, b2_handle build_ch
                                       int32_t nbuild_out, b2_handle* out);
 /* mixed join: an extra non-equi condition (BOOL8 program bound over [stream columns ++ build columns]) decides which
  * equi-matched pairs survive — Table.mixed{Inner,Left,LeftSemi,LeftAnti}JoinGatherMap(s) (GpuHashJoin.scala:335-600),
- * ConditionalHashJoinIterator (:1556).  Inner / left outer / left semi / left anti. */
+ * ConditionalHashJoinIterator (:1556).  Inner / left outer / left semi / left anti / right outer / full outer; right outer and
+ * full outer mark the build rows of the passing pairs in a tracker and emit the others after the last stream batch. */
 int b2_exec_join_set_condition(b2_handle join, b2_handle condition_program);
 /* GpuSubPartitionHashJoin (GpuShuffledHashJoinExec.scala:228-281, GpuSubPartitionHashJoin.scala:86-617): when the build side
  * passes target_bytes (table_bytes; raised to 16 KiB) both sides are split into num_partitions (2..256; Spark default 16,
  * RapidsConf.scala:2660) spillable buckets by murmur3 seed 100 of the join keys and joined bucket by bucket; adjacent small
- * buckets are packed up to the target, a bucket still over it (FULL OUTER: by its build or its stream side) is split once
+ * buckets are packed up to the target, a bucket still over it (FULL OUTER without a condition: by its build or its stream
+ * side) is split once
  * more (seed 110) and then joined as it is, so the rows of a single key must fit on the device.  Without this call, or when the build side stays within target_bytes,
  * the join is unchanged. */
 int b2_exec_join_set_sub_partitioning(b2_handle join, int64_t target_bytes, int32_t num_partitions);

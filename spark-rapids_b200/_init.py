@@ -25,7 +25,7 @@ OP_STARTS_WITH, OP_ENDS_WITH, OP_CONTAINS, OP_LIKE, OP_SUBSTRING = 50, 51, 52, 5
 # b2_agg_kind
 AGG_SUM, AGG_COUNT, AGG_MIN, AGG_MAX, AGG_COUNT_ALL = 1, 2, 3, 4, 5
 # b2_join_kind
-JOIN_INNER, JOIN_LEFT_OUTER, JOIN_LEFT_SEMI, JOIN_LEFT_ANTI, JOIN_FULL_OUTER = 0, 1, 2, 3, 4
+JOIN_INNER, JOIN_LEFT_OUTER, JOIN_LEFT_SEMI, JOIN_LEFT_ANTI, JOIN_FULL_OUTER, JOIN_RIGHT_OUTER = 0, 1, 2, 3, 4, 5
 
 
 def _ptr(a):
@@ -542,7 +542,8 @@ class JoinHashTable:
         self.h = ctypes.c_int64(out.value)
 
     def probe(self, probe_keys, kind=JOIN_INNER, selection=None):
-        """-> (left_map Column, right_map Column|None); selection: INT32 row ids of probe_keys (filter_row_ids) that take part"""
+        """-> (left_map Column, right_map Column|None); selection: INT32 row ids of probe_keys (filter_row_ids) that take part.
+        JOIN_RIGHT_OUTER: the inner maps, then (INT32_MIN, b) for every build row b no probe row matched, ascending"""
         lm, rm = ctypes.c_int64(), ctypes.c_int64()
         check(lib.b2_join_probe_sel(self.h, probe_keys.h, selection.h if selection is not None else 0, kind, ctypes.byref(lm), ctypes.byref(rm)))
         return Column(lm.value), (Column(rm.value) if rm.value else None)
@@ -557,6 +558,39 @@ class JoinHashTable:
     def __del__(self):
         if getattr(self, "h", None) is not None and self.h.value:
             lib.b2_join_hash_table_close(self.h)
+            self.h = ctypes.c_int64(0)
+
+
+class JoinTracker:
+    """one bit per build row of `table` (a JoinHashTable): the build rows that found a partner across probe batches, for outer
+    joins that preserve the build side"""
+
+    def __init__(self, table):
+        out = ctypes.c_int64()
+        check(lib.b2_join_tracker_create(table.h, ctypes.byref(out)))
+        self.h = ctypes.c_int64(out.value)
+        self._table = table   # the bits stand for its build rows
+
+    def probe(self, table, probe_keys, kind=JOIN_INNER, selection=None):
+        """table.probe (kind JOIN_INNER or JOIN_LEFT_OUTER) that also marks every build row it finds"""
+        lm, rm = ctypes.c_int64(), ctypes.c_int64()
+        check(lib.b2_join_probe_track(table.h, probe_keys.h, selection.h if selection is not None else 0, kind, self.h, ctypes.byref(lm),
+                                      ctypes.byref(rm)))
+        return Column(lm.value), Column(rm.value)
+
+    def mark(self, right_map, passed=None):
+        """marks right_map[i] where passed[i] (BOOL8 Column, NULL = false; None: every i); negative entries are skipped"""
+        check(lib.b2_join_tracker_mark(self.h, right_map.h, passed.h if passed is not None else 0))
+
+    def unmatched(self):
+        """INT32 Column: the build rows never marked, ascending"""
+        out = ctypes.c_int64()
+        check(lib.b2_join_tracker_unmatched(self.h, ctypes.byref(out)))
+        return Column(out.value)
+
+    def __del__(self):
+        if getattr(self, "h", None) is not None and self.h.value:
+            lib.b2_join_tracker_close(self.h)
             self.h = ctypes.c_int64(0)
 
 

@@ -29,7 +29,8 @@ Table* scan_aggregate(const Program* prog, bool has_pred, const Table* t, const 
 Program* make_passthrough_program(const Table* t, const std::vector<int>& cols);
 Table* filter_select(const Program* prog, const Table* t, const int32_t* keep, int nkeep);
 Column* filter_row_ids(const Program* prog, const Table* t);
-bool join_probe_pred(b2_handle ht, const Table* batch, int key_col, const Program* prog, Column** out_lm, Column** out_rm, int64_t* npass_out);   // join.cu
+bool join_probe_pred(b2_handle ht, const Table* batch, int key_col, const Program* prog, Column** out_lm, Column** out_rm, int64_t* npass_out,
+                     b2_handle tracker);   // join.cu
 Table* filter_by_mask(const Table* t, Column* m);
 Column* rows_with_passing_pair(const Column* left_map, const Column* pass, int64_t stream_rows, bool invert);
 
@@ -610,7 +611,36 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
   std::vector<int> stream_out, build_out;    // pruned: the columns each side contributes (in this order)
   TableRef build_table;
   b2_handle ht = 0;
-  ~GpuShuffledHashJoinExec() { if (ht) b2_join_hash_table_close(ht); }
+  // Outer joins that preserve the build side — RIGHT OUTER, and FULL OUTER with a condition — are "tracked" (HashOuterJoinIterator,
+  // GpuHashJoin.scala:1807-1814): stream batches are joined one at a time (INNER / the conditional LEFT OUTER), a tracker over
+  // the hash table keeps the build rows that found a partner, and once the stream side is exhausted the others come out
+  // with NULL stream columns (getFinalBatch, :2288-2326).  FULL OUTER without a condition coalesces its stream side instead.
+  b2_handle tracker = 0;
+  TableRef stream_schema;                       // zero rows of the stream columns: the NULL side of the final rows
+  Column* fin_ids = nullptr;                    // ascending ids of the unmatched build rows
+  std::deque<std::pair<int64_t, int64_t>> fin;  // ranges of fin_ids still to emit
+  bool fin_started = false;
+  ~GpuShuffledHashJoinExec() {
+    if (fin_ids) col_release(fin_ids);
+    if (tracker) b2_join_tracker_close(tracker);
+    if (ht) b2_join_hash_table_close(ht);
+  }
+  bool tracked() const { return kind == B2_JOIN_RIGHT_OUTER || (kind == B2_JOIN_FULL_OUTER && condition); }
+  bool coalesced() const { return kind == B2_JOIN_FULL_OUTER && !condition; }
+  void new_tracker() {   // after (re)building ht
+    if (tracker) { b2_join_tracker_close(tracker); tracker = 0; }
+    fin_started = false;
+    if (!tracked()) return;
+    int rc = b2_join_tracker_create(ht, &tracker);
+    if (rc != B2_OK) throw Error(rc, b2_last_error());
+  }
+  // the maps of one stream batch (through a selection vector): RIGHT OUTER probes INNER and marks the build rows it finds
+  void probe(const Table* keys, Column* sel, b2_handle* lm, b2_handle* rm) {
+    const b2_handle sh = sel ? to_handle(sel) : 0;
+    int rc = kind == B2_JOIN_RIGHT_OUTER ? b2_join_probe_track(ht, to_handle(const_cast<Table*>(keys)), sh, B2_JOIN_INNER, tracker, lm, rm)
+                                         : b2_join_probe_sel(ht, to_handle(const_cast<Table*>(keys)), sh, kind, lm, rm);
+    if (rc != B2_OK) throw Error(rc, b2_last_error());
+  }
   static Table* select(const Table* t, const std::vector<int>& idx) {
     std::vector<Column*> cols;
     for (int i : idx) { if (i < 0 || i >= (int)t->cols.size()) throw Error(B2_ERR_INVALID, "join key index out of range"); col_incref(t->cols[i]); cols.push_back(t->cols[i]); }
@@ -627,9 +657,11 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
     if (parts.empty()) throw Error(B2_ERR_UNSUPPORTED, "empty build side needs the build schema");
     if (parts.size() == 1) build_table = std::move(parts[0]);
     else { std::vector<const Table*> ts; for (auto& p : parts) ts.push_back(p.t); build_table = TableRef(concat_tables(ts)); }
+    parts.clear();   // the batches are not needed once concatenated: the hash table does not wait for them to go
     TableRef bk(select(build_table.t, build_keys));
     int rc = b2_join_build(to_handle(bk.t), nulls_equal, &ht);
     if (rc != B2_OK) throw Error(rc, b2_last_error());
+    new_tracker();
     built = true;
   }
   // A GpuFilterExec directly below the stream side is fused by late materialisation: the filter yields a selection vector
@@ -648,8 +680,15 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
     Owned plm, prm, sel;
     int64_t npass = 0;
     bool in_probe = false;
-    if (kind == B2_JOIN_INNER && keys.size() == 1) {
-      try { in_probe = join_probe_pred(ht, raw.t, keys[0], program_from(fused->program), &plm.c, &prm.c, &npass); }
+    if (tracked() && !stream_schema.t) {
+      std::vector<int> fcols;
+      const int n = fused->keep.empty() ? (int)raw.t->cols.size() : (int)fused->keep.size();
+      for (int c = 0; c < n; c++) fcols.push_back(raw_col(c));
+      TableRef cols(select(raw.t, fcols));
+      stream_schema = TableRef(slice_table(cols.t, 0, 0));
+    }
+    if ((kind == B2_JOIN_INNER || kind == B2_JOIN_RIGHT_OUTER) && keys.size() == 1) {
+      try { in_probe = join_probe_pred(ht, raw.t, keys[0], program_from(fused->program), &plm.c, &prm.c, &npass, tracker); }
       catch (const Error& e) { if (!splittable(e)) throw; in_probe = false; }   // memory pressure: the selection-vector path retries and splits
     }
     auto make_sel = [&] { if (!sel.c) sel.c = run_as(fused, [&] { return filter_row_ids(program_from(fused->program), raw.t); }); };
@@ -665,8 +704,7 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
           make_sel();
           TableRef sk(select(raw.t, keys));
           b2_handle lm = 0, rm = 0;
-          int rc = b2_join_probe_sel(ht, to_handle(sk.t), to_handle(sel.c), kind, &lm, &rm);
-          if (rc != B2_OK) throw Error(rc, b2_last_error());
+          probe(sk.t, sel.c, &lm, &rm);
           lmc = col_from(lm); rmc = rm ? col_from(rm) : nullptr;
         }
         ColGuard lmap(lmc);
@@ -695,17 +733,21 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
   }
   Table* do_next() override {
     if (!todo.empty()) return drain_todo();
+    if (!fin.empty()) return final_next();
     if (!built) build();
     if (sp_active) return sp_next();
     if (!fusion_checked) {
       fusion_checked = true;
       if (kind != B2_JOIN_FULL_OUTER && !condition && !getenv("B2_NO_FILTER_FUSION")) fused = dynamic_cast<GpuFilterExec*>(children[0]);
     }
-    if (fused) return fused_next();
+    if (fused) {
+      if (Table* t = fused_next()) return t;
+      return tracked() ? final_start() : nullptr;
+    }
     TableRef s;
-    if (kind == B2_JOIN_FULL_OUTER) {
-      // the unmatched build rows can only be emitted once every stream row has been seen: the stream side is
-      // coalesced into one batch (the reference tracks matched build rows across batches instead)
+    if (coalesced()) {
+      // the unmatched build rows can only be emitted once every stream row has been seen: without a condition the stream
+      // side is coalesced into one batch (tracked joins keep the matched build rows across batches instead: final_start)
       if (full_done) return nullptr;
       full_done = true;
       std::vector<TableRef> parts;
@@ -716,9 +758,55 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
     } else {
       s = TableRef(children[0]->next());
     }
-    if (!s.t) return nullptr;
+    if (!s.t) return tracked() ? final_start() : nullptr;
+    if (tracked() && !stream_schema.t) stream_schema = TableRef(slice_table(s.t, 0, 0));
     todo.emplace_back(std::move(s), 0);
     return drain_todo();
+  }
+  // Tracked joins, after the last stream batch (of the pair, when sub-partitioned): the build rows never marked, NULL on the
+  // stream side.  A gather that does not fit (B2_ERR_OOM after retries, B2_ERR_SIZE_OVERFLOW) is halved, so these rows may
+  // come in several batches.
+  Table* final_start() {
+    if (fin_started) return nullptr;
+    fin_started = true;
+    if (!(sp_active ? sp_stream_empty.t : stream_schema.t))
+      throw Error(B2_ERR_UNSUPPORTED, "empty stream side of an outer join that preserves the build side needs the stream schema");
+    if (fin_ids) { col_release(fin_ids); fin_ids = nullptr; }
+    fin_ids = with_retry([&] {
+      b2_handle h = 0;
+      int rc = b2_join_tracker_unmatched(tracker, &h);
+      if (rc != B2_OK) throw Error(rc, b2_last_error());
+      return col_from(h);
+    });
+    if (fin_ids->size) fin.emplace_back(0, fin_ids->size);
+    return fin.empty() ? nullptr : final_next();
+  }
+  Table* final_next() {
+    while (true) {
+      const std::pair<int64_t, int64_t> r = fin.front();
+      fin.pop_front();
+      try {
+        return with_retry([&] { return final_rows(r.first, r.second); });
+      } catch (const Error& e) {
+        if (!splittable(e) || r.second - r.first < 2) throw;
+        note_split();
+        const int64_t mid = r.first + (r.second - r.first) / 2;
+        fin.emplace_front(mid, r.second);
+        fin.emplace_front(r.first, mid);
+      }
+    }
+  }
+  Table* final_rows(int64_t lo, int64_t hi) {
+    const Table* ss = sp_active ? sp_stream_empty.t : stream_schema.t;
+    const int64_t n = hi - lo;
+    std::vector<int> scols;
+    if (pruned) scols = stream_out;
+    else for (int c = 0; c < (int)ss->cols.size(); c++) scols.push_back(c);
+    ColGuard oob(new_column(B2_INT32, 0, n, false));
+    if (n) CUDA_CHECK(cudaMemsetAsync(oob.c->data.p, 0x80, (size_t)n * 4, stream()));   // 0x80808080 < 0: out of bounds -> NULL row
+    TableRef left(gather_table(ss, oob.c->data.as<int32_t>(), n, true, &scols));
+    TableRef right(gather_table(build_table.t, fin_ids->data.as<int32_t>() + lo, n, false, pruned ? &build_out : nullptr));
+    return concat_cols(left.t, right.t);
   }
   // stream slices waiting to be joined (a batch that had to be split leaves its halves here; one output per next())
   std::deque<std::pair<TableRef, int>> todo;
@@ -733,7 +821,7 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
       try {
         return with_retry([&] { return join_batch(st.t); });
       } catch (const Error& e) {
-        if (!splittable(e) || st.t->rows < 2 || depth >= 16 || kind == B2_JOIN_FULL_OUTER) throw;
+        if (!splittable(e) || st.t->rows < 2 || depth >= 16 || coalesced()) throw;
         note_split();
         const int64_t mid = st.t->rows / 2;
         TableRef lo, hi;
@@ -767,7 +855,6 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
   }
   // equi-join pairs -> condition over the pair rows -> per join type
   Table* join_batch_conditional(const Table* st) {
-    if (kind == B2_JOIN_FULL_OUTER) throw Error(B2_ERR_UNSUPPORTED, "full outer join with a non-equi condition");
     TableRef sk(select(st, stream_keys));
     b2_handle lm = 0, rm = 0;
     int rc = b2_join_probe(ht, to_handle(sk.t), B2_JOIN_INNER, &lm, &rm);
@@ -783,13 +870,17 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
     TableRef pt(from_handle_owned(ph));
     Column* pass = pt.t->cols[0];
     if (pass->dtype != B2_BOOL8) throw Error(B2_ERR_INVALID, "join condition must be BOOL8");
+    if (tracker) {   // the build rows of the pairs that pass (marking is idempotent: a retried or halved batch sets the same bits)
+      rc = b2_join_tracker_mark(tracker, to_handle(rmap.c), to_handle(pass));
+      if (rc != B2_OK) throw Error(rc, b2_last_error());
+    }
     auto stream_side = [&](const Table* t) {   // semi / anti output: the node's stream columns
       std::vector<Column*> cols;
       if (pruned) for (int c : stream_out) { col_incref(t->cols[c]); cols.push_back(t->cols[c]); }
       else for (auto* c : t->cols) { col_incref(c); cols.push_back(c); }
       return new_table(std::move(cols));
     };
-    if (kind == B2_JOIN_INNER) {
+    if (kind == B2_JOIN_INNER || kind == B2_JOIN_RIGHT_OUTER) {
       TableRef out(prune_pairs(pairs.t, nstream));
       return filter_by_mask(out.t, pass);
     }
@@ -798,7 +889,7 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
       TableRef side(stream_side(st));
       return filter_by_mask(side.t, flags.c);
     }
-    // LEFT OUTER: the passing pairs, then every stream row without one, NULL on the build side
+    // LEFT OUTER (and FULL OUTER's per-batch part): the passing pairs, then every stream row without one, NULL on the build side
     TableRef pruned_pairs(prune_pairs(pairs.t, nstream));
     TableRef matched(filter_by_mask(pruned_pairs.t, pass));
     ColGuard lonely(rows_with_passing_pair(lmap.c, pass, st->rows, true));
@@ -816,8 +907,7 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
     if (condition) return join_batch_conditional(st);
     TableRef sk(select(st, stream_keys));
     b2_handle lm = 0, rm = 0;
-    int rc = b2_join_probe(ht, to_handle(sk.t), kind, &lm, &rm);
-    if (rc != B2_OK) throw Error(rc, b2_last_error());
+    probe(sk.t, nullptr, &lm, &rm);
     ColGuard lmap(col_from(lm));
     ColGuard rmap(rm ? col_from(rm) : nullptr);
     TableRef left(gather_table(st, lmap.c->data.as<int32_t>(), lmap.c->size, kind == B2_JOIN_FULL_OUTER, pruned ? &stream_out : nullptr));
@@ -930,20 +1020,22 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
       split_into(raw.t, sel.c ? sel.c->data.as<int32_t>() : nullptr, sel.c ? sel.c->size : raw.t->rows, keys, keep, SP_SEED, sp_parts,
                  first_level, false, &sp_stats[3]);
     }
-    if (!sp_stream_empty.t && kind == B2_JOIN_FULL_OUTER) throw Error(B2_ERR_UNSUPPORTED, "empty stream side of a full outer join needs the stream schema");
+    if (!sp_stream_empty.t && (coalesced() || tracked()))
+      throw Error(B2_ERR_UNSUPPORTED, "empty stream side of an outer join that preserves the build side needs the stream schema");
   }
   bool useless(const Bucket& b) const {
     if (kind == B2_JOIN_INNER || kind == B2_JOIN_LEFT_SEMI) return b.build.empty() || b.stream.empty();
     if (kind == B2_JOIN_FULL_OUTER) return b.build.empty() && b.stream.empty();
+    if (kind == B2_JOIN_RIGHT_OUTER) return b.build.empty();   // build rows without stream rows are still output
     return b.stream.empty();   // LEFT OUTER / ANTI: stream rows without build rows are still output
   }
-  // GpuSubPartitionPairIterator: a bucket still over the target is split once more, with its stream pieces.  FULL OUTER
-  // coalesces a pair's stream side, so there a bucket whose stream pieces pass the target is split again as well.
+  // GpuSubPartitionPairIterator: a bucket still over the target is split once more, with its stream pieces.  FULL OUTER without
+  // a condition coalesces a pair's stream side, so there a bucket whose stream pieces pass the target is split again as well.
   void repartition() {
     Bucket b = std::move(sp_buckets.front());
     sp_buckets.pop_front();
     sp_stats[1]++;
-    const int64_t bytes = std::max(b.build_bytes, kind == B2_JOIN_FULL_OUTER ? b.stream_bytes : 0);
+    const int64_t bytes = std::max(b.build_bytes, coalesced() ? b.stream_bytes : 0);
     const int k2 = (int)std::min<int64_t>(256, std::max<int64_t>(sp_parts, bytes / sp_target + 1));
     std::vector<Bucket> sub(k2);
     auto second_level = [&](int p) -> Bucket& { return sub[p]; };
@@ -955,12 +1047,14 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
     for (int p = k2 - 1; p >= 0; p--) { sub[p].resplit = true; sp_buckets.push_front(std::move(sub[p])); }
   }
   // GpuBatchSubPartitionIterator: the next pair = adjacent useful buckets whose build pieces together stay within the target.
-  // Builds its hash table and queues its stream pieces in probe groups of at most the target (FULL OUTER: one group).
+  // Builds its hash table (and tracker) and queues its stream pieces in probe groups of at most the target (FULL OUTER without a
+  // condition: one group).
   bool open_next_pair() {
+    if (tracker) { b2_join_tracker_close(tracker); tracker = 0; }
     if (ht) { b2_join_hash_table_close(ht); ht = 0; }
     build_table.reset();
     auto over = [&](const Bucket& b) {
-      return !b.resplit && (b.build_bytes > sp_target || (kind == B2_JOIN_FULL_OUTER && b.stream_bytes > sp_target));
+      return !b.resplit && (b.build_bytes > sp_target || (coalesced() && b.stream_bytes > sp_target));
     };
     while (!sp_buckets.empty()) {
       if (useless(sp_buckets.front())) sp_buckets.pop_front();
@@ -968,8 +1062,8 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
       else break;
     }
     if (sp_buckets.empty()) return false;
-    // FULL OUTER coalesces the pair's stream side as well, so its stream pieces count against the target too
-    const bool full = kind == B2_JOIN_FULL_OUTER;
+    // FULL OUTER without a condition coalesces the pair's stream side as well, so its stream pieces count against the target too
+    const bool full = coalesced();
     std::vector<Bucket> pair;
     int64_t bytes = sp_buckets.front().build_bytes, sbytes = sp_buckets.front().stream_bytes;
     pair.push_back(std::move(sp_buckets.front()));
@@ -996,7 +1090,8 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
       if (rc != B2_OK) throw Error(rc, b2_last_error());
       return h;
     });
-    if (kind == B2_JOIN_FULL_OUTER) { sp_probe.push_back(std::move(sps)); return true; }
+    new_tracker();
+    if (full) { sp_probe.push_back(std::move(sps)); return true; }
     std::vector<SpillPiece> grp;
     int64_t gb = 0, gr = 0;
     for (auto& p : sps) {
@@ -1011,10 +1106,15 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
     if (!sp_read) { sp_read = true; split_stream_side(); }
     while (true) {
       if (!todo.empty()) return drain_todo();
+      if (!fin.empty()) return final_next();
       if (!sp_probe.empty()) {
         std::vector<SpillPiece> grp = std::move(sp_probe.front());
         sp_probe.pop_front();
         todo.emplace_back(TableRef(concat_pieces(grp, sp_stream_empty.t)), 0);
+        continue;
+      }
+      if (ht && tracked() && !fin_started) {   // the pair's last group is done (or it had none): its unmatched build rows
+        if (Table* t = final_start()) return t;
         continue;
       }
       if (!open_next_pair()) return nullptr;

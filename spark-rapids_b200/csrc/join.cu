@@ -95,6 +95,17 @@ __device__ __forceinline__ uint64_t join_entry(const uint64_t* __restrict__ slot
   return slots[idx];
 }
 
+// Matched build rows across stream batches (RIGHT OUTER, and FULL OUTER with a condition): a JoinTracker holds one bit per build
+// row of one hash table, and the tracking (TRACK) probe variants set bit br where they find build row br — inside the probe,
+// where the reference filters the gather map, copies it, scatters it into a BOOL8 tracker and rebuilds the tracker per batch
+// (HashJoinStreamSideIterator.updateTrackingMask, GpuHashJoin.scala:2164-2204).  The word is read first and the atomic issued
+// only when the bit is clear: in FK -> PK joins many stream rows hit the same build row, and neighbouring build rows share a word.
+__device__ __forceinline__ void track_hit(uint32_t* __restrict__ bits, int32_t br) {
+  uint32_t* w = bits + ((uint32_t)br >> 5);
+  const uint32_t b = 1u << (br & 31);
+  if (!(*w & b)) atomicOr(w, b);
+}
+
 // single pass for a distinct build side: at most one match per stream row.
 //   INNER: pairs appended with ONE atomic per warp and PI x 32 rows (join output order is unspecified: docs/compatibility.md:18-25)
 //   LEFT OUTER: row r -> (r, match or INT32_MIN), no compaction at all
@@ -103,11 +114,12 @@ __device__ __forceinline__ uint64_t join_entry(const uint64_t* __restrict__ slot
 // the output range of a whole chunk is reserved with a single atomic (the per-32-rows atomic on one address was the
 // serialisation point of the kernel: ~10 M same-address atomics per TPC-H q3 step).
 constexpr int PI = 8;
+template <bool TRACK>
 __global__ void __launch_bounds__(256) join_probe_distinct_kernel(const __grid_constant__ KeyCols probe, const __grid_constant__ KeyCols build, int64_t n,
                                            const uint64_t* __restrict__ slots, uint32_t mask, bool nulls_equal,
                                            bool fast, int kind, unsigned long long* __restrict__ total, int32_t* __restrict__ left_map,
                                            int32_t* __restrict__ right_map, const unsigned long long* __restrict__ bloom, uint32_t bloom_mask,
-                                           const int32_t* __restrict__ sel) {
+                                           const int32_t* __restrict__ sel, uint32_t* __restrict__ track) {
   const int lane = threadIdx.x & 31;
   const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
   for (int64_t base = warp * (32 * PI); base < n; base += nwarps * (32 * PI)) {
@@ -154,6 +166,10 @@ __global__ void __launch_bounds__(256) join_probe_distinct_kernel(const __grid_c
         }
         idx = (idx + 1) & mask;
       }
+    }
+    if constexpr (TRACK) {
+#pragma unroll
+      for (int j = 0; j < PI; j++) if (br[j] != INT32_MIN) track_hit(track, br[j]);
     }
     if (kind == B2_JOIN_LEFT_OUTER) {
 #pragma unroll
@@ -225,11 +241,11 @@ struct L2Persist {
 // (Tried and measured slower on the q3 step: evict-first loads of the selection vector and the key column plus
 // evict-last Bloom words.  Unlike part_scatter2 — hash.cu — nothing here is half-written and waiting in L2.)
 constexpr int PQ = 8;
-template <typename K>
+template <typename K, bool TRACK>
 __device__ __forceinline__ void probe_distinct1_rows(const K* __restrict__ keys, const int32_t (&r)[PQ], const uint64_t* __restrict__ slots,
                                                      uint32_t mask, const unsigned long long* __restrict__ bloom, uint32_t bloom_mask,
                                                      unsigned long long* __restrict__ total, int32_t* __restrict__ left_map,
-                                                     int32_t* __restrict__ right_map, int32_t* s_q) {
+                                                     int32_t* __restrict__ right_map, int32_t* s_q, uint32_t* __restrict__ track) {
   typedef typename std::make_unsigned<K>::type UK;
   const int lane = threadIdx.x & 31;
   const uint32_t lt = (1u << lane) - 1u;
@@ -285,19 +301,22 @@ __device__ __forceinline__ void probe_distinct1_rows(const K* __restrict__ keys,
       unsigned long long o = 0;
       if (lane == 0) o = atomicAdd(total, (unsigned long long)__popc(b));
       o = __shfl_sync(0xffffffffu, o, 0) + __popc(b & lt);
-      if (hit) { left_map[o] = src; right_map[o] = br; }
+      if (hit) {
+        left_map[o] = src; right_map[o] = br;
+        if constexpr (TRACK) track_hit(track, br);
+      }
     }
   }
   __syncwarp();   // the queue is rewritten by the next call
 }
 
 // every row of the batch (SEL = false) or the rows of a selection vector (a filter below the join emitted row ids)
-template <typename K, bool SEL>
+template <typename K, bool SEL, bool TRACK>
 __global__ void __launch_bounds__(256) join_probe_distinct1_kernel(const K* __restrict__ keys, const int32_t* __restrict__ sel, int64_t n,
                                                                    const uint64_t* __restrict__ slots, uint32_t mask,
                                                                    const unsigned long long* __restrict__ bloom, uint32_t bloom_mask,
                                                                    unsigned long long* __restrict__ total, int32_t* __restrict__ left_map,
-                                                                   int32_t* __restrict__ right_map) {
+                                                                   int32_t* __restrict__ right_map, uint32_t* __restrict__ track) {
   __shared__ int32_t s_q[8][32 * PQ];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
@@ -308,7 +327,7 @@ __global__ void __launch_bounds__(256) join_probe_distinct1_kernel(const K* __re
       const int64_t rr = base + j * 32 + lane;
       r[j] = rr < n ? (SEL ? sel[rr] : (int32_t)rr) : -1;
     }
-    probe_distinct1_rows<K>(keys, r, slots, mask, bloom, bloom_mask, total, left_map, right_map, s_q[w]);
+    probe_distinct1_rows<K, TRACK>(keys, r, slots, mask, bloom, bloom_mask, total, left_map, right_map, s_q[w], track);
   }
 }
 
@@ -326,12 +345,13 @@ __global__ void __launch_bounds__(256) join_probe_distinct1_kernel(const K* __re
 // 3 measured slower, 5 spills).
 constexpr int FP_TILE = 8 * 1024, FP_WORDS = FP_TILE / 32, FP_CTAS = 4;
 static_assert(FP_WORDS == SF_NT, "one mask word per thread");
-template <typename K>
+template <typename K, bool TRACK>
 __global__ void __launch_bounds__(SF_NT, FP_CTAS) join_filter_probe_kernel(const __grid_constant__ SimplePred sp, const K* __restrict__ keys, int64_t n,
                                                                           const uint64_t* __restrict__ slots, uint32_t mask,
                                                                           const unsigned long long* __restrict__ bloom, uint32_t bloom_mask,
                                                                           unsigned long long* __restrict__ total, int32_t* __restrict__ left_map,
-                                                                          int32_t* __restrict__ right_map, unsigned long long* __restrict__ npass) {
+                                                                          int32_t* __restrict__ right_map, unsigned long long* __restrict__ npass,
+                                                                          uint32_t* __restrict__ track) {
   __shared__ uint32_t s_mask[FP_WORDS];
   __shared__ uint16_t s_rows[FP_TILE];               // offsets in the tile of the passing rows, ascending
   __shared__ int32_t s_q[SF_NT / 32][32 * PQ];
@@ -360,19 +380,20 @@ __global__ void __launch_bounds__(SF_NT, FP_CTAS) join_filter_probe_kernel(const
         const int q = q0 + j * 32 + lane;
         r[j] = q < qn ? (int32_t)(row0 + s_rows[q]) : -1;
       }
-      probe_distinct1_rows<K>(keys, r, slots, mask, bloom, bloom_mask, total, left_map, right_map, s_q[w]);
+      probe_distinct1_rows<K, TRACK>(keys, r, slots, mask, bloom, bloom_mask, total, left_map, right_map, s_q[w], track);
     }
     __syncthreads();   // s_mask, s_rows and s_wtot are rewritten by the next tile
   }
 }
 
-// MODE 0: count matches per probe row; MODE 1: write pairs at offsets
-template <int MODE>
+// MODE 0: count matches per probe row; MODE 1: write pairs at offsets (TRACK: and mark the build rows)
+template <int MODE, bool TRACK = false>
 __global__ void join_probe_kernel(const __grid_constant__ KeyCols probe, const __grid_constant__ KeyCols build, int64_t n,
                                   const uint64_t* __restrict__ slots, uint32_t mask, bool nulls_equal,
                                   bool fast, int kind, int32_t* __restrict__ counts, const int64_t* __restrict__ offsets,
                                   int32_t* __restrict__ left_map, int32_t* __restrict__ right_map,
-                                  const unsigned long long* __restrict__ bloom, uint32_t bloom_mask, const int32_t* __restrict__ sel) {
+                                  const unsigned long long* __restrict__ bloom, uint32_t bloom_mask, const int32_t* __restrict__ sel,
+                                  uint32_t* __restrict__ track) {
   for (int64_t rr = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; rr < n; rr += (int64_t)gridDim.x * blockDim.x) {
     const int64_t r = sel ? (int64_t)sel[rr] : rr;   // see join_probe_distinct_kernel
     int32_t matches = 0;
@@ -391,7 +412,10 @@ __global__ void join_probe_kernel(const __grid_constant__ KeyCols probe, const _
         if ((uint32_t)(e >> 32) == h) {
           const int32_t br = (int32_t)(uint32_t)e;
           if (fast ? (ek == kb) : rows_equal(probe, r, build, br, nulls_equal)) {
-            if (MODE == 1 && !semi_like) { left_map[o + matches] = (int32_t)r; right_map[o + matches] = br; }
+            if (MODE == 1 && !semi_like) {
+              left_map[o + matches] = (int32_t)r; right_map[o + matches] = br;
+              if constexpr (TRACK) track_hit(track, br);
+            }
             matches++;
             if (semi_like) break;
           }
@@ -414,20 +438,136 @@ __global__ void join_probe_kernel(const __grid_constant__ KeyCols probe, const _
   }
 }
 
-// ---- full outer = left outer + the build rows no stream row matched (GpuHashJoin.scala full-join gather maps) -----
-__global__ void mark_matched_kernel(const int32_t* __restrict__ right_map, int64_t n, uint8_t* __restrict__ matched) {
+// ---- the tracker's other two kernels: marking through a gather map, and the ids of the clear bits -------------------
+// tracker_mark_kernel: bit right_map[i] for every i whose pass[i] is true (BOOL8, NULL = false; no pass = every i).  Negative
+// entries (INT32_MIN, OutOfBoundsPolicy.NULLIFY) are skipped; an entry >= nb sets *bad.  Serves conditional joins, where only
+// the pairs that pass the condition count.
+__global__ void tracker_mark_kernel(const int32_t* __restrict__ right_map, const int8_t* __restrict__ pass, const uint32_t* __restrict__ pass_valid,
+                                    int64_t n, int64_t nb, uint32_t* __restrict__ bits, int32_t* __restrict__ bad) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     const int32_t r = right_map[i];
-    if (r >= 0) matched[r] = 1;
+    if (r < 0 || (pass && !(pass[i] && row_valid(pass_valid, i)))) continue;
+    if (r >= nb) { *bad = 1; continue; }
+    track_hit(bits, r);
   }
 }
-__global__ void unmatched_flags_kernel(const uint8_t* __restrict__ matched, int64_t nb, int32_t* __restrict__ flags) {
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < nb; i += (int64_t)gridDim.x * blockDim.x) flags[i] = matched[i] ? 0 : 1;
+
+// tracker_unmatched (HashOuterJoinIterator.getFinalBatch, GpuHashJoin.scala:2288-2326): the bitmap -> ascending INT32 ids of
+// its clear bits.  A tile is TU_NT x TU_WPT words (65536 build rows); count pass (popcount of the complemented words, tail word
+// masked) -> exclusive_scan of the tile counts -> write pass.  In the write pass warp w of a tile owns 32 x TU_WPT consecutive
+// words and takes them 32 at a time (lane = word, so the ids come out ascending); a round's ids (<= 1024) are staged in shared
+// memory and leave as aligned 16-byte vectors.  Bytes: nb / 8 read twice, 4 per unmatched row written (8 with `left_fill`).
+constexpr int TU_NT = 256, TU_WPT = 8, TU_TILE = TU_NT * TU_WPT;
+__device__ __forceinline__ uint32_t clear_bits(const uint32_t* __restrict__ bits, int64_t i, int64_t nwords, uint32_t tail) {
+  if (i >= nwords) return 0u;
+  const uint32_t m = ~bits[i];
+  return i == nwords - 1 ? m & tail : m;
 }
-__global__ void append_unmatched_kernel(const uint8_t* __restrict__ matched, const int32_t* __restrict__ pos, int64_t nb, int64_t base,
-                                        int32_t* __restrict__ left_map, int32_t* __restrict__ right_map) {
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < nb; i += (int64_t)gridDim.x * blockDim.x)
-    if (!matched[i]) { left_map[base + pos[i]] = INT32_MIN; right_map[base + pos[i]] = (int32_t)i; }
+__global__ void __launch_bounds__(TU_NT) tracker_count_kernel(const uint32_t* __restrict__ bits, int64_t nwords, uint32_t tail,
+                                                              int32_t* __restrict__ counts) {
+  __shared__ int32_t s_w[TU_NT / 32];
+  const int64_t w0 = (int64_t)blockIdx.x * TU_TILE;
+  int c = 0;
+#pragma unroll
+  for (int j = 0; j < TU_WPT; j++) c += __popc(clear_bits(bits, w0 + j * TU_NT + threadIdx.x, nwords, tail));
+  c = __reduce_add_sync(0xffffffffu, c);
+  if ((threadIdx.x & 31) == 0) s_w[threadIdx.x >> 5] = c;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int t = 0;
+#pragma unroll
+    for (int k = 0; k < TU_NT / 32; k++) t += s_w[k];
+    counts[blockIdx.x] = t;
+  }
+}
+// the warp's `cnt` staged values to dst[0..cnt): single elements up to the first 16-byte boundary of dst, then aligned
+// vectors, then the tail (dst 4-byte aligned)
+template <typename V>
+__device__ __forceinline__ void warp_store_aligned(int32_t* __restrict__ dst, int cnt, int lane, V&& value) {
+  const int head = min(cnt, (int)(((16 - ((uintptr_t)dst & 15)) & 15) >> 2));
+  for (int k = lane; k < head; k += 32) dst[k] = value(k);
+  const int nv = (cnt - head) >> 2;
+  for (int v = lane; v < nv; v += 32) {
+    const int k = head + 4 * v;
+    *reinterpret_cast<int4*>(dst + k) = make_int4(value(k), value(k + 1), value(k + 2), value(k + 3));
+  }
+  for (int k = head + 4 * nv + lane; k < cnt; k += 32) dst[k] = value(k);
+}
+__global__ void __launch_bounds__(TU_NT) tracker_write_kernel(const uint32_t* __restrict__ bits, int64_t nwords, uint32_t tail,
+                                                              const int32_t* __restrict__ offs, int32_t* __restrict__ ids,
+                                                              int32_t* __restrict__ left_fill) {
+  __shared__ int32_t s_stage[TU_NT / 32][32 * 32];
+  __shared__ int32_t s_wt[TU_NT / 32];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int64_t w0 = (int64_t)blockIdx.x * TU_TILE + w * (32 * TU_WPT);   // this warp's first word
+  uint32_t m[TU_WPT];
+  int tot = 0;
+#pragma unroll
+  for (int j = 0; j < TU_WPT; j++) { m[j] = clear_bits(bits, w0 + j * 32 + lane, nwords, tail); tot += __popc(m[j]); }
+  tot = __reduce_add_sync(0xffffffffu, tot);
+  if (lane == 0) s_wt[w] = tot;
+  __syncthreads();
+  int64_t g = offs[blockIdx.x];
+  for (int k = 0; k < w; k++) g += s_wt[k];
+  int32_t* st = s_stage[w];
+#pragma unroll
+  for (int j = 0; j < TU_WPT; j++) {
+    const int c = __popc(m[j]);
+    int inc = c;
+    for (int o = 1; o < 32; o <<= 1) { const int x = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += x; }
+    const int cnt = __shfl_sync(0xffffffffu, inc, 31);
+    if (cnt == 0) continue;
+    int pos = inc - c;
+    const int32_t row0 = (int32_t)((w0 + j * 32 + lane) * 32);
+    for (uint32_t mm = m[j]; mm; mm &= mm - 1) st[pos++] = row0 + __ffs(mm) - 1;
+    __syncwarp();
+    warp_store_aligned(ids + g, cnt, lane, [&](int k) { return st[k]; });
+    if (left_fill) warp_store_aligned(left_fill + g, cnt, lane, [](int) { return INT32_MIN; });
+    __syncwarp();   // the stage is rewritten by the next round
+    g += cnt;
+  }
+}
+
+struct JoinTracker {
+  const void* table;   // the JoinTable whose build rows the bits stand for
+  int64_t nb;
+  DevBuf bits;         // uint32 [ceil(nb / 32)], zeroed at creation
+  DevBuf bad;          // int32: tracker_mark_kernel saw an entry >= nb
+};
+static JoinTracker* tracker_new(const void* table, int64_t nb) {
+  std::unique_ptr<JoinTracker> tr(new JoinTracker());
+  tr->table = table; tr->nb = nb;
+  tr->bits = DevBuf((size_t)std::max<int64_t>((nb + 31) / 32, 1) * 4);
+  tr->bad = DevBuf(4);
+  CUDA_CHECK(cudaMemsetAsync(tr->bits.p, 0, tr->bits.bytes, stream()));
+  CUDA_CHECK(cudaMemsetAsync(tr->bad.p, 0, 4, stream()));
+  return tr.release();
+}
+static void tracker_mark(JoinTracker* tr, const int32_t* right_map, int64_t n, const Column* pass) {
+  if (n)
+    launch("tracker_mark_kernel", tracker_mark_kernel, grid_for(n, 256), 256, 0, stream(), right_map, pass ? pass->data.as<int8_t>() : nullptr,
+           pass ? pass->validity() : nullptr, n, tr->nb, tr->bits.as<uint32_t>(), tr->bad.as<int32_t>());
+}
+// count pass + scan: the number of clear bits; `offs` keeps the tile offsets for tracker_unmatched_write
+static int64_t tracker_unmatched_count(const JoinTracker* tr, DevBuf& offs) {
+  const int64_t nwords = (tr->nb + 31) / 32, ntiles = (nwords + TU_TILE - 1) / TU_TILE;
+  offs = DevBuf((size_t)(ntiles + 1) * 4);
+  if (!ntiles) return 0;
+  const uint32_t tail = (tr->nb & 31) ? (1u << (tr->nb & 31)) - 1u : 0xffffffffu;
+  launch("tracker_count_kernel", tracker_count_kernel, (int)ntiles, TU_NT, 0, stream(), tr->bits.as<uint32_t>(), nwords, tail, offs.as<int32_t>());
+  exclusive_scan<int32_t, int32_t>(offs.as<int32_t>(), offs.as<int32_t>(), ntiles, true);
+  int32_t u = 0;
+  d2h(&u, offs.as<int32_t>() + ntiles, 1);
+  sync();
+  return u;
+}
+// write pass: the ascending ids to ids[0..u), and INT32_MIN to left_fill[0..u) when given
+static void tracker_unmatched_write(const JoinTracker* tr, const DevBuf& offs, int64_t u, int32_t* ids, int32_t* left_fill) {
+  if (!u) return;
+  const int64_t nwords = (tr->nb + 31) / 32, ntiles = (nwords + TU_TILE - 1) / TU_TILE;
+  const uint32_t tail = (tr->nb & 31) ? (1u << (tr->nb & 31)) - 1u : 0xffffffffu;
+  launch("tracker_write_kernel", tracker_write_kernel, (int)ntiles, TU_NT, 0, stream(), tr->bits.as<uint32_t>(), nwords, tail, offs.as<int32_t>(), ids,
+         left_fill);
 }
 
 // ---- mixed (conditional) joins: which stream rows own at least one pair that passes the join condition ------------------------
@@ -455,14 +595,26 @@ static JoinTable* jt_from(b2_handle h) {
   if (!h) throw Error(B2_ERR_INVALID, "null hash table handle");
   return reinterpret_cast<JoinTable*>((intptr_t)h);
 }
+static JoinTracker* tracker_from(b2_handle h) {
+  if (!h) throw Error(B2_ERR_INVALID, "null join tracker handle");
+  return reinterpret_cast<JoinTracker*>((intptr_t)h);
+}
 
 // GpuFilter directly below the stream side of an INNER FK -> PK join, fused INTO the probe (join_filter_probe_kernel) when
 // the predicate is of the simple shape (simplefilter.cuh) and the probe qualifies for the one-key distinct probe: the gather
 // maps carry ORIGINAL row ids of `batch`, `npass_out` = rows that passed the filter (the filter node's numOutputRows).
+// tracker != 0: the build rows found are marked in it (join_filter_probe_kernel's tracking variant).
 // false = not applicable, the caller takes the selection-vector path (b2_filter_row_ids + b2_join_probe_sel).
-bool join_probe_pred(b2_handle ht, const Table* batch, int key_col, const Program* prog, Column** out_lm, Column** out_rm, int64_t* npass_out) {
+bool join_probe_pred(b2_handle ht, const Table* batch, int key_col, const Program* prog, Column** out_lm, Column** out_rm, int64_t* npass_out,
+                     b2_handle tracker) {
   if (getenv("B2_JOIN_NO_FAST_PROBE")) return false;
   JoinTable* jt = jt_from(ht);
+  uint32_t* track = nullptr;
+  if (tracker) {
+    JoinTracker* tr = tracker_from(tracker);
+    if (tr->table != jt) throw Error(B2_ERR_INVALID, "join tracker belongs to another hash table");
+    track = tr->bits.as<uint32_t>();
+  }
   const int64_t n = batch->rows;
   if (!jt->distinct || !jt->fast || jt->key_idx.size() != 1 || n < (1 << 16) || n >= 0x7fffffffLL) return false;
   if (key_col < 0 || key_col >= (int)batch->cols.size()) throw Error(B2_ERR_INVALID, "join key index out of range");
@@ -480,10 +632,19 @@ bool join_probe_pred(b2_handle ht, const Table* batch, int key_col, const Progra
     const uint64_t* sl = jt->slots.as<uint64_t>(); const uint32_t msk = (uint32_t)(jt->cap - 1);
     const unsigned long long* bl = jt->bloom.as<unsigned long long>();
     unsigned long long* tp = tot.as<unsigned long long>();
-    if (pw == 8) launch("join_filter_probe_kernel", join_filter_probe_kernel<int64_t>, grid, SF_NT, 0, stream(), sp, pc->data.as<int64_t>(), n, sl, msk, bl,
-                        jt->bloom_mask, tp, lm.c->data.as<int32_t>(), rm.c->data.as<int32_t>(), tp + 1);
-    else launch("join_filter_probe_kernel", join_filter_probe_kernel<int32_t>, grid, SF_NT, 0, stream(), sp, pc->data.as<int32_t>(), n, sl, msk, bl,
-                jt->bloom_mask, tp, lm.c->data.as<int32_t>(), rm.c->data.as<int32_t>(), tp + 1);
+    int32_t* lp = lm.c->data.as<int32_t>(); int32_t* rp = rm.c->data.as<int32_t>();
+    if (track) {
+      if (pw == 8) launch("join_filter_probe_track_kernel", join_filter_probe_kernel<int64_t, true>, grid, SF_NT, 0, stream(), sp, pc->data.as<int64_t>(), n,
+                          sl, msk, bl, jt->bloom_mask, tp, lp, rp, tp + 1, track);
+      else launch("join_filter_probe_track_kernel", join_filter_probe_kernel<int32_t, true>, grid, SF_NT, 0, stream(), sp, pc->data.as<int32_t>(), n, sl,
+                  msk, bl, jt->bloom_mask, tp, lp, rp, tp + 1, track);
+    } else if (pw == 8) {
+      launch("join_filter_probe_kernel", join_filter_probe_kernel<int64_t, false>, grid, SF_NT, 0, stream(), sp, pc->data.as<int64_t>(), n, sl, msk, bl,
+             jt->bloom_mask, tp, lp, rp, tp + 1, nullptr);
+    } else {
+      launch("join_filter_probe_kernel", join_filter_probe_kernel<int32_t, false>, grid, SF_NT, 0, stream(), sp, pc->data.as<int32_t>(), n, sl, msk, bl,
+             jt->bloom_mask, tp, lp, rp, tp + 1, nullptr);
+    }
   }
   unsigned long long h[2] = {0, 0};
   d2h(h, tot.p, 2);
@@ -563,7 +724,7 @@ int b2_join_probe_filter(b2_handle ht, b2_handle table, int32_t key_col, b2_hand
   B2_CHECK(key_col >= 0 && key_col < (int)t->cols.size(), "join key index out of range");
   Column* lm = nullptr; Column* rm = nullptr;
   int64_t npass = 0;
-  if (join_probe_pred(ht, t, key_col, program_from(predicate_program), &lm, &rm, &npass)) {
+  if (join_probe_pred(ht, t, key_col, program_from(predicate_program), &lm, &rm, &npass, 0)) {
     *out_left_map = to_handle(lm); *out_right_map = to_handle(rm); *out_npass = npass;
     return B2_OK;
   }
@@ -583,54 +744,22 @@ int b2_join_probe(b2_handle ht, b2_handle probe_keys_table, int32_t kind, b2_han
   return b2_join_probe_sel(ht, probe_keys_table, 0, kind, out_left_map, out_right_map);
 }
 
-// probe through a selection vector: `selection` (INT32 row ids into probe_keys_table, ascending, e.g. from b2_filter_row_ids)
-// names the stream rows that take part; the left gather map carries ORIGINAL row ids of probe_keys_table's batch
-int b2_join_probe_sel(b2_handle ht, b2_handle probe_keys_table, b2_handle selection, int32_t kind, b2_handle* out_left_map, b2_handle* out_right_map) {
-  B2_TRY
-  JoinTable* jt = jt_from(ht);
-  Table* pt = table_from(probe_keys_table);
+}  // extern "C"
+
+namespace b2 {
+// The probe proper: kinds INNER .. LEFT_ANTI, through an optional selection vector; track != nullptr (INNER / LEFT OUTER only)
+// takes the tracking variant of whichever probe kernel runs.
+static void probe_maps(JoinTable* jt, Table* pt, b2_handle selection, int32_t kind, uint32_t* track, b2_handle* out_left_map, b2_handle* out_right_map) {
   const int32_t* sel = nullptr;
   int64_t nsel = 0;
   if (selection) {
     Column* sc = col_from(selection);
     B2_CHECK(sc->dtype == B2_INT32, "selection vector must be INT32");
-    B2_CHECK(kind != B2_JOIN_FULL_OUTER, "full outer join through a selection vector");
     sel = sc->data.as<int32_t>(); nsel = sc->size;
   }
   B2_CHECK(pt->cols.size() == jt->keys->cols.size(), "probe and build key counts differ");
   for (size_t i = 0; i < pt->cols.size(); i++)
     B2_CHECK(pt->cols[i]->dtype == jt->keys->cols[i]->dtype, "probe and build key dtypes differ");
-  if (kind == B2_JOIN_FULL_OUTER) {
-    // left outer maps, then one extra row (left = out of bounds -> NULLs) per build row that nothing matched
-    B2_CHECK(out_right_map != nullptr, "a full outer join needs both gather maps");
-    b2_handle hl = 0, hr = 0;
-    int rc = b2_join_probe_sel(ht, probe_keys_table, 0, B2_JOIN_LEFT_OUTER, &hl, &hr);
-    if (rc != B2_OK) return rc;
-    ColGuard lo(col_from(hl)), ro(col_from(hr));
-    const int64_t m = lo.c->size, nb = jt->keys->rows;
-    DevBuf matched((size_t)std::max<int64_t>(nb, 1)), pos((size_t)(nb + 1) * 4);
-    CUDA_CHECK(cudaMemsetAsync(matched.p, 0, matched.bytes, stream()));
-    int32_t extra = 0;
-    if (nb) {
-      if (m) launch(mark_matched_kernel, grid_for(m, 256), 256, 0, stream(), ro.c->data.as<int32_t>(), m, matched.as<uint8_t>());
-      launch(unmatched_flags_kernel, grid_for(nb, 256), 256, 0, stream(), matched.as<uint8_t>(), nb, pos.as<int32_t>());
-      exclusive_scan<int32_t, int32_t>(pos.as<int32_t>(), pos.as<int32_t>(), nb, true);
-      d2h(&extra, pos.as<int32_t>() + nb, 1);
-      sync();
-    }
-    if (m + extra > 0x7fffffffLL) throw Error(B2_ERR_SIZE_OVERFLOW, "join output exceeds 2^31-1 rows; split the stream batch");
-    ColGuard lm(new_column(B2_INT32, 0, m + extra, false)), rm(new_column(B2_INT32, 0, m + extra, false));
-    if (m) {
-      CUDA_CHECK(cudaMemcpyAsync(lm.c->data.p, lo.c->data.p, (size_t)m * 4, cudaMemcpyDeviceToDevice, stream()));
-      CUDA_CHECK(cudaMemcpyAsync(rm.c->data.p, ro.c->data.p, (size_t)m * 4, cudaMemcpyDeviceToDevice, stream()));
-    }
-    if (extra)
-      launch(append_unmatched_kernel, grid_for(nb, 256), 256, 0, stream(), matched.as<uint8_t>(), pos.as<int32_t>(), nb, m, lm.c->data.as<int32_t>(),
-             rm.c->data.as<int32_t>());
-    *out_left_map = to_handle(lm.release());
-    *out_right_map = to_handle(rm.release());
-    return B2_OK;
-  }
   B2_CHECK(kind >= B2_JOIN_INNER && kind <= B2_JOIN_LEFT_ANTI, "bad join kind");
   // an empty selection vector has no data buffer (sel == nullptr) and selects no row
   const int64_t n = selection ? nsel : pt->rows;
@@ -653,29 +782,38 @@ int b2_join_probe_sel(b2_handle ht, b2_handle probe_keys_table, b2_handle select
         const uint64_t* sl = jt->slots.as<uint64_t>(); const uint32_t msk = (uint32_t)(jt->cap - 1);
         const unsigned long long* bl = jt->bloom.as<unsigned long long>(); unsigned long long* tp = tot.as<unsigned long long>();
         int32_t* lp = lm.c->data.as<int32_t>(); int32_t* rp = rm.c->data.as<int32_t>();
-        if (pw == 8)
-          launch("join_probe_distinct1_kernel", sel ? join_probe_distinct1_kernel<int64_t, true> : join_probe_distinct1_kernel<int64_t, false>, grid, 256, 0,
-                 stream(), pc->data.as<int64_t>(), sel, n, sl, msk, bl, jt->bloom_mask, tp, lp, rp);
-        else
-          launch("join_probe_distinct1_kernel", sel ? join_probe_distinct1_kernel<int32_t, true> : join_probe_distinct1_kernel<int32_t, false>, grid, 256, 0,
-                 stream(), pc->data.as<int32_t>(), sel, n, sl, msk, bl, jt->bloom_mask, tp, lp, rp);
+        if (track) {
+          if (pw == 8)
+            launch("join_probe_distinct1_track_kernel", sel ? join_probe_distinct1_kernel<int64_t, true, true> : join_probe_distinct1_kernel<int64_t, false, true>,
+                   grid, 256, 0, stream(), pc->data.as<int64_t>(), sel, n, sl, msk, bl, jt->bloom_mask, tp, lp, rp, track);
+          else
+            launch("join_probe_distinct1_track_kernel", sel ? join_probe_distinct1_kernel<int32_t, true, true> : join_probe_distinct1_kernel<int32_t, false, true>,
+                   grid, 256, 0, stream(), pc->data.as<int32_t>(), sel, n, sl, msk, bl, jt->bloom_mask, tp, lp, rp, track);
+        } else if (pw == 8) {
+          launch("join_probe_distinct1_kernel", sel ? join_probe_distinct1_kernel<int64_t, true, false> : join_probe_distinct1_kernel<int64_t, false, false>,
+                 grid, 256, 0, stream(), pc->data.as<int64_t>(), sel, n, sl, msk, bl, jt->bloom_mask, tp, lp, rp, nullptr);
+        } else {
+          launch("join_probe_distinct1_kernel", sel ? join_probe_distinct1_kernel<int32_t, true, false> : join_probe_distinct1_kernel<int32_t, false, false>,
+                 grid, 256, 0, stream(), pc->data.as<int32_t>(), sel, n, sl, msk, bl, jt->bloom_mask, tp, lp, rp, nullptr);
+        }
       } else {
-        launch("join_probe_distinct_kernel", join_probe_distinct_kernel, grid_for(n, 256), 256, 0, stream(), pk, bk, n, jt->slots.as<uint64_t>(),
-               (uint32_t)(jt->cap - 1), jt->nulls_equal, jt->fast, kind, tot.as<unsigned long long>(), lm.c->data.as<int32_t>(), rm.c->data.as<int32_t>(),
-               jt->bloom.as<unsigned long long>(), jt->bloom_mask, sel);
+        launch(track ? "join_probe_distinct_track_kernel" : "join_probe_distinct_kernel",
+               track ? join_probe_distinct_kernel<true> : join_probe_distinct_kernel<false>, grid_for(n, 256), 256, 0, stream(), pk, bk, n,
+               jt->slots.as<uint64_t>(), (uint32_t)(jt->cap - 1), jt->nulls_equal, jt->fast, kind, tot.as<unsigned long long>(), lm.c->data.as<int32_t>(),
+               rm.c->data.as<int32_t>(), jt->bloom.as<unsigned long long>(), jt->bloom_mask, sel, track);
       }
       if (kind == B2_JOIN_INNER) { unsigned long long h = 0; d2h(&h, tot.p, 1); sync(); matched = (int64_t)h; }
     }
     lm.c->size = matched; rm.c->size = matched;  // buffers stay sized for n rows
     *out_left_map = to_handle(lm.release());
     if (out_right_map) *out_right_map = to_handle(rm.release()); else col_release(rm.release());
-    return B2_OK;
+    return;
   }
   DevBuf counts((size_t)std::max<int64_t>(n, 1) * 4), offsets((size_t)(n + 1) * 8);
   int64_t total = 0;
   if (n) {
     launch("join_probe_count_kernel", join_probe_kernel<0>, grid_for(n, 256), 256, 0, stream(), pk, bk, n, jt->slots.as<uint64_t>(), (uint32_t)(jt->cap - 1),
-           jt->nulls_equal, jt->fast, kind, counts.as<int32_t>(), nullptr, nullptr, nullptr, jt->bloom.as<unsigned long long>(), jt->bloom_mask, sel);
+           jt->nulls_equal, jt->fast, kind, counts.as<int32_t>(), nullptr, nullptr, nullptr, jt->bloom.as<unsigned long long>(), jt->bloom_mask, sel, nullptr);
     exclusive_scan<int32_t, int64_t>(counts.as<int32_t>(), offsets.as<int64_t>(), n, true);
     d2h(&total, offsets.as<int64_t>() + n, 1);
     sync();
@@ -686,11 +824,108 @@ int b2_join_probe_sel(b2_handle ht, b2_handle probe_keys_table, b2_handle select
   ColGuard lm(new_column(B2_INT32, 0, total, false));
   ColGuard rm(semi_like ? nullptr : new_column(B2_INT32, 0, total, false));
   if (n && total)
-    launch("join_probe_write_kernel", join_probe_kernel<1>, grid_for(n, 256), 256, 0, stream(), pk, bk, n, jt->slots.as<uint64_t>(), (uint32_t)(jt->cap - 1),
-           jt->nulls_equal, jt->fast, kind, nullptr, offsets.as<int64_t>(), lm.c->data.as<int32_t>(), semi_like ? nullptr : rm.c->data.as<int32_t>(),
-           jt->bloom.as<unsigned long long>(), jt->bloom_mask, sel);
+    launch(track ? "join_probe_write_track_kernel" : "join_probe_write_kernel", track ? join_probe_kernel<1, true> : join_probe_kernel<1, false>,
+           grid_for(n, 256), 256, 0, stream(), pk, bk, n, jt->slots.as<uint64_t>(), (uint32_t)(jt->cap - 1), jt->nulls_equal, jt->fast, kind, nullptr,
+           offsets.as<int64_t>(), lm.c->data.as<int32_t>(), semi_like ? nullptr : rm.c->data.as<int32_t>(), jt->bloom.as<unsigned long long>(),
+           jt->bloom_mask, sel, track);
   *out_left_map = to_handle(lm.release());
   if (out_right_map) *out_right_map = semi_like ? 0 : to_handle(rm.release());
+}
+
+// maps (lo, ro) of m rows, then (INT32_MIN, b) for every build row b whose bit is clear in `tr`, ascending
+static void append_unmatched(const JoinTracker* tr, const Column* lo, const Column* ro, b2_handle* out_left_map, b2_handle* out_right_map) {
+  const int64_t m = lo->size;
+  DevBuf offs;
+  const int64_t extra = tracker_unmatched_count(tr, offs);
+  if (m + extra > 0x7fffffffLL) throw Error(B2_ERR_SIZE_OVERFLOW, "join output exceeds 2^31-1 rows; split the stream batch");
+  ColGuard lm(new_column(B2_INT32, 0, m + extra, false)), rm(new_column(B2_INT32, 0, m + extra, false));
+  if (m) {
+    CUDA_CHECK(cudaMemcpyAsync(lm.c->data.p, lo->data.p, (size_t)m * 4, cudaMemcpyDeviceToDevice, stream()));
+    CUDA_CHECK(cudaMemcpyAsync(rm.c->data.p, ro->data.p, (size_t)m * 4, cudaMemcpyDeviceToDevice, stream()));
+  }
+  tracker_unmatched_write(tr, offs, extra, rm.c->data.as<int32_t>() + m, lm.c->data.as<int32_t>() + m);
+  *out_left_map = to_handle(lm.release());
+  *out_right_map = to_handle(rm.release());
+}
+}  // namespace b2
+
+extern "C" {
+
+// probe through a selection vector: `selection` (INT32 row ids into probe_keys_table, ascending, e.g. from b2_filter_row_ids)
+// names the stream rows that take part; the left gather map carries ORIGINAL row ids of probe_keys_table's batch
+int b2_join_probe_sel(b2_handle ht, b2_handle probe_keys_table, b2_handle selection, int32_t kind, b2_handle* out_left_map, b2_handle* out_right_map) {
+  B2_TRY
+  JoinTable* jt = jt_from(ht);
+  Table* pt = table_from(probe_keys_table);
+  if (kind == B2_JOIN_FULL_OUTER || kind == B2_JOIN_RIGHT_OUTER) {
+    // FULL OUTER: the left outer maps; RIGHT OUTER: the inner maps (marking the build rows found as it goes).  Then one extra
+    // row (left = out of bounds -> NULLs) per build row that nothing matched, ascending
+    B2_CHECK(out_right_map != nullptr, "an outer join that preserves the build side needs both gather maps");
+    B2_CHECK(!(selection && kind == B2_JOIN_FULL_OUTER), "full outer join through a selection vector");
+    std::unique_ptr<JoinTracker> tr(tracker_new(jt, jt->keys->rows));
+    b2_handle hl = 0, hr = 0;
+    if (kind == B2_JOIN_FULL_OUTER) probe_maps(jt, pt, 0, B2_JOIN_LEFT_OUTER, nullptr, &hl, &hr);
+    else probe_maps(jt, pt, selection, B2_JOIN_INNER, tr->bits.as<uint32_t>(), &hl, &hr);
+    ColGuard lo(col_from(hl)), ro(col_from(hr));
+    if (kind == B2_JOIN_FULL_OUTER) tracker_mark(tr.get(), ro.c->data.as<int32_t>(), ro.c->size, nullptr);
+    append_unmatched(tr.get(), lo.c, ro.c, out_left_map, out_right_map);
+    return B2_OK;
+  }
+  probe_maps(jt, pt, selection, kind, nullptr, out_left_map, out_right_map);
+  B2_CATCH
+}
+
+int b2_join_tracker_create(b2_handle ht, b2_handle* out_tracker) {
+  B2_TRY
+  JoinTable* jt = jt_from(ht);
+  *out_tracker = to_handle(tracker_new(jt, jt->build_rows));
+  B2_CATCH
+}
+
+int b2_join_tracker_close(b2_handle tracker) {
+  B2_TRY
+  delete tracker_from(tracker);
+  B2_CATCH
+}
+
+int b2_join_probe_track(b2_handle ht, b2_handle probe_keys_table, b2_handle selection, int32_t kind, b2_handle tracker, b2_handle* out_left_map,
+                        b2_handle* out_right_map) {
+  B2_TRY
+  JoinTable* jt = jt_from(ht);
+  JoinTracker* tr = tracker_from(tracker);
+  B2_CHECK(tr->table == jt, "join tracker belongs to another hash table");
+  B2_CHECK(kind == B2_JOIN_INNER || kind == B2_JOIN_LEFT_OUTER, "only inner and left outer probes write the maps a tracker follows");
+  B2_CHECK(out_right_map != nullptr, "a tracked probe needs both gather maps");
+  probe_maps(jt, table_from(probe_keys_table), selection, kind, tr->bits.as<uint32_t>(), out_left_map, out_right_map);
+  B2_CATCH
+}
+
+int b2_join_tracker_mark(b2_handle tracker, b2_handle right_map, b2_handle pass) {
+  B2_TRY
+  JoinTracker* tr = tracker_from(tracker);
+  const Column* rm = col_from(right_map);
+  B2_CHECK(rm->dtype == B2_INT32, "right gather map must be INT32");
+  const Column* pc = pass ? col_from(pass) : nullptr;
+  B2_CHECK(!pc || (pc->dtype == B2_BOOL8 && pc->size == rm->size), "pass mask must be BOOL8 with one row per map entry");
+  tracker_mark(tr, rm->data.as<int32_t>(), rm->size, pc);
+  int32_t bad = 0;
+  d2h(&bad, tr->bad.p, 1);
+  sync();
+  if (bad) {
+    CUDA_CHECK(cudaMemsetAsync(tr->bad.p, 0, 4, stream()));
+    throw Error(B2_ERR_INVALID, "right gather map entry past the build side");
+  }
+  B2_CATCH
+}
+
+int b2_join_tracker_unmatched(b2_handle tracker, b2_handle* out_ids) {
+  B2_TRY
+  const JoinTracker* tr = tracker_from(tracker);
+  DevBuf offs;
+  const int64_t u = tracker_unmatched_count(tr, offs);
+  ColGuard ids(new_column(B2_INT32, 0, u, false));
+  tracker_unmatched_write(tr, offs, u, ids.c->data.as<int32_t>(), nullptr);
+  *out_ids = to_handle(ids.release());
   B2_CATCH
 }
 

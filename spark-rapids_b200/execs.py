@@ -167,7 +167,9 @@ def GpuHashAggregateExec(child, grouping, aggregates, pre_project=None, conditio
 
 def GpuShuffledHashJoinExec(stream_keys, build_keys, join_type, stream, build, nulls_equal=False, stream_out=None, build_out=None, condition=None,
                             target_bytes=None, num_sub_partitions=16):
-    """stream_out / build_out: columns a pruning GpuProjectExec above the join keeps (fused into the gathers);
+    """join_type JOIN_RIGHT_OUTER keeps every build row (stream columns NULL where no stream row matched): Spark's RightOuter
+    with BuildRight, or LeftOuter with BuildLeft with the children swapped;
+    stream_out / build_out: columns a pruning GpuProjectExec above the join keeps (fused into the gathers);
     condition: non-equi join condition (Expr / Program) bound over [stream columns ++ build columns] (mixed join);
     target_bytes given: GpuSubPartitionHashJoin, a build side larger than target_bytes is split into num_sub_partitions
     spillable buckets with the stream side and joined bucket by bucket (the build side need not fit on the device)"""
@@ -220,5 +222,8 @@ def GpuBroadcastExchangeExec(child, comm=None, rank=0, world=1):
 
 
 def GpuBroadcastHashJoinExec(stream_keys, build_keys, join_type, stream, build, comm=None, rank=0, world=1, **kw):
-    """GpuBroadcastHashJoinExecBase.scala: the build side is broadcast, the stream side stays where it is (no shuffle)"""
+    """GpuBroadcastHashJoinExecBase.scala: the build side is broadcast, the stream side stays where it is (no shuffle).
+    JOIN_RIGHT_OUTER is refused: every rank would emit the unmatched build rows (Spark never broadcasts the preserved side)"""
+    if join_type == m.JOIN_RIGHT_OUTER:
+        raise ValueError("a broadcast hash join cannot preserve its build side (JOIN_RIGHT_OUTER)")
     return GpuShuffledHashJoinExec(stream_keys, build_keys, join_type, stream, GpuBroadcastExchangeExec(build, comm, rank, world), **kw)
