@@ -488,6 +488,10 @@ int b2_exec_join_set_condition(b2_handle join, b2_handle condition_program);
 int b2_exec_join_set_sub_partitioning(b2_handle join, int64_t target_bytes, int32_t num_partitions);
 /* out4: first-level buckets (0 = not sub-partitioned), buckets repartitioned, build bytes split, stream bytes split */
 int b2_exec_join_sub_partition_stats(b2_handle join, int64_t* out4);
+/* out3: stream batches whose output rows the filter-probe kernel wrote (the emitting probe of an INNER FK -> PK join with a
+ * simple filter below its stream side), batches joined through gather maps, and emitted batches whose matches passed the
+ * estimated output size and were joined again through the maps (counted among the maps batches as well) */
+int b2_exec_join_emit_stats(b2_handle join, int64_t* out3);
 /* GpuBroadcastExchangeExec (GpuBroadcastExchangeExec.scala): every rank gets the whole child relation, one batch.  Used as
  * the build child of a join it makes GpuBroadcastHashJoinExec (GpuBroadcastHashJoinExecBase.scala:1-203). */
 int b2_exec_broadcast_exchange(b2_handle child, b2_handle comm, int32_t rank, int32_t world, b2_handle* out);

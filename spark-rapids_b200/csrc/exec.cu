@@ -18,7 +18,9 @@
 //   GpuShuffleExchangeExec    GpuShuffleExchangeExecBase.scala:384-536 with the NCCL all-to-all
 #include <algorithm>
 #include <chrono>
+#include <cmath>
 #include <deque>
+#include "joinemit.cuh"
 #include "vm.cuh"
 
 namespace b2 {
@@ -670,6 +672,36 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
   GpuFilterExec* fused = nullptr;
   bool fusion_checked = false;
   int raw_col(int filter_out_col) const { return fused->keep.empty() ? filter_out_col : fused->keep[filter_out_col]; }
+  // Emitting probe (join_probe_pred_emit): the maps and the payload gathers of a filtered FK -> PK join replaced by output rows
+  // written from the probe kernel.  The output size is known only after the probe, and GpuCoalesceBatches above holds every
+  // output batch, so columns of the batch's row count are out of the question: the first batch goes through the maps and
+  // gives the matches per stream row, later batches get columns of cap = min(n, ceil(1.1 * max ratio seen * n) + 65536) rows,
+  // and a batch whose matches pass cap is joined again through the maps (only the speed depends on the estimate).
+  JoinPayload em_payload;
+  bool em_packed = false, em_ok = false;   // payload packed (or tried); usable
+  double em_ratio = -1;                    // most matches per stream row of a batch so far; < 0: no batch joined yet
+  int64_t em_stats[3] = {0, 0, 0};         // batches emitted, batches joined through maps, overflow reruns
+  void note_matches(int64_t matches, int64_t rows) { if (rows > 0) em_ratio = std::max(em_ratio, (double)matches / (double)rows); }
+  // the output of stream batch `raw` written by the probe; nullptr: join it through the maps
+  Table* try_emit(const Table* raw, int key_col, const std::vector<int>& stream_cols, int64_t* npass) {
+    if (kind != B2_JOIN_INNER || tracker || em_ratio < 0 || getenv("B2_JOIN_NO_EMIT")) return nullptr;
+    if (!em_packed) {
+      em_packed = true;
+      std::vector<int> bcols = build_out;
+      if (!pruned) for (int c = 0; c < (int)build_table.t->cols.size(); c++) bcols.push_back(c);
+      try { em_ok = join_pack_payload(build_table.t, bcols, em_payload); }
+      catch (const Error& e) { if (e.code != B2_ERR_OOM) throw; em_ok = false; em_payload = JoinPayload(); }   // no room: the maps
+    }
+    if (!em_ok) return nullptr;
+    const int64_t n = raw->rows;
+    const int64_t cap = std::min<int64_t>(n, (int64_t)std::ceil(1.1 * em_ratio * (double)n) + 65536);
+    Table* out = nullptr;
+    int64_t total = 0;
+    if (!join_probe_pred_emit(ht, raw, key_col, program_from(fused->program), stream_cols, em_payload, cap, &out, &total, npass)) return nullptr;
+    note_matches(total, n);
+    if (!out) em_stats[2]++;
+    return out;
+  }
   Table* fused_next() {
     TableRef raw(fused->children[0]->next());
     if (!raw.t) return nullptr;
@@ -687,17 +719,21 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
       TableRef cols(select(raw.t, fcols));
       stream_schema = TableRef(slice_table(cols.t, 0, 0));
     }
-    if ((kind == B2_JOIN_INNER || kind == B2_JOIN_RIGHT_OUTER) && keys.size() == 1) {
-      try { in_probe = join_probe_pred(ht, raw.t, keys[0], program_from(fused->program), &plm.c, &prm.c, &npass, tracker); }
-      catch (const Error& e) { if (!splittable(e)) throw; in_probe = false; }   // memory pressure: the selection-vector path retries and splits
-    }
-    auto make_sel = [&] { if (!sel.c) sel.c = run_as(fused, [&] { return filter_row_ids(program_from(fused->program), raw.t); }); };
-    if (!in_probe) make_sel();
-    fused->num_output_rows += in_probe ? npass : sel.c->size; fused->num_output_batches++;
     if (pruned) for (int c : stream_out) left_cols.push_back(raw_col(c));
     else { const int n = fused->keep.empty() ? (int)raw.t->cols.size() : (int)fused->keep.size(); for (int c = 0; c < n; c++) left_cols.push_back(raw_col(c)); }
+    TableRef emitted;
+    if ((kind == B2_JOIN_INNER || kind == B2_JOIN_RIGHT_OUTER) && keys.size() == 1) {
+      try {
+        emitted = TableRef(try_emit(raw.t, keys[0], left_cols, &npass));
+        if (!emitted.t) in_probe = join_probe_pred(ht, raw.t, keys[0], program_from(fused->program), &plm.c, &prm.c, &npass, tracker);
+      } catch (const Error& e) { if (!splittable(e)) throw; in_probe = false; }   // memory pressure: the selection-vector path retries and splits
+    }
+    auto make_sel = [&] { if (!sel.c) sel.c = run_as(fused, [&] { return filter_row_ids(program_from(fused->program), raw.t); }); };
+    if (!in_probe && !emitted.t) make_sel();
+    fused->num_output_rows += in_probe || emitted.t ? npass : sel.c->size; fused->num_output_batches++;
+    if (emitted.t) { em_stats[0]++; return emitted.release(); }
     try {
-      return with_retry([&]() -> Table* {
+      Table* out = with_retry([&]() -> Table* {
         Column* lmc = nullptr; Column* rmc = nullptr;
         if (plm.c) { lmc = plm.take(); rmc = prm.take(); }   // the maps of the fused kernel (first attempt only)
         else {
@@ -709,6 +745,7 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
         }
         ColGuard lmap(lmc);
         ColGuard rmap(rmc);
+        note_matches(lmap.c->size, raw.t->rows);
         TableRef left(gather_table(raw.t, lmap.c->data.as<int32_t>(), lmap.c->size, false, &left_cols));
         if (!rmap.c || (pruned && build_out.empty())) return left.release();
         TableRef right(gather_table(build_table.t, rmap.c->data.as<int32_t>(), rmap.c->size, kind == B2_JOIN_LEFT_OUTER, pruned ? &build_out : nullptr));
@@ -719,6 +756,8 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
         left.t->cols.clear(); right.t->cols.clear();
         return new_table(std::move(cols));
       });
+      em_stats[1]++;
+      return out;
     } catch (const Error& e) {
       if (!splittable(e)) throw;
       // memory pressure / 2^31 limit: materialise the filter output after all and take the split-and-retry path
@@ -819,7 +858,9 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
       const int depth = todo.front().second;
       todo.pop_front();
       try {
-        return with_retry([&] { return join_batch(st.t); });
+        Table* out = with_retry([&] { return join_batch(st.t); });
+        em_stats[1]++;
+        return out;
       } catch (const Error& e) {
         if (!splittable(e) || st.t->rows < 2 || depth >= 16 || coalesced()) throw;
         note_split();
@@ -1682,6 +1723,13 @@ int b2_exec_join_sub_partition_stats(b2_handle join, int64_t* out4) {
   auto* j = dynamic_cast<GpuShuffledHashJoinExec*>(exec_from(join));
   B2_CHECK(j, "not a hash join node");
   for (int i = 0; i < 4; i++) out4[i] = j->sp_stats[i];
+  B2_CATCH
+}
+int b2_exec_join_emit_stats(b2_handle join, int64_t* out3) {
+  B2_TRY
+  auto* j = dynamic_cast<GpuShuffledHashJoinExec*>(exec_from(join));
+  B2_CHECK(j, "not a hash join node");
+  for (int i = 0; i < 3; i++) out3[i] = j->em_stats[i];
   B2_CATCH
 }
 int b2_exec_broadcast_exchange(b2_handle child, b2_handle comm, int32_t rank, int32_t world, b2_handle* out) {

@@ -9,6 +9,7 @@
 // (8-byte slots: 32-bit hash tag + 32-bit build row) that any number of probe calls reuse.
 // Probe is count -> scan -> write so the gather maps are exactly sized and ordered by stream row.
 #include <type_traits>
+#include "joinemit.cuh"
 #include "prim.cuh"
 #include "rowops.cuh"
 #include "simplefilter.cuh"
@@ -241,11 +242,63 @@ struct L2Persist {
 // (Tried and measured slower on the q3 step: evict-first loads of the selection vector and the key column plus
 // evict-last Bloom words.  Unlike part_scatter2 — hash.cu — nothing here is half-written and waiting in L2.)
 constexpr int PQ = 8;
-template <typename K, bool TRACK>
+
+// The output row descriptors of the emitting probe (EMIT): instead of the gather maps, a lane that finds build row br for
+// stream row src writes the joined row itself at the offset it reserved — the stream columns loaded at src (the key column
+// from the probed key, no load), the build columns unpacked from one aligned 8- or 16-byte load of the packed payload at br
+// (JoinPayload).  Offsets at or past `cap` are counted and not written: the caller sizes the output from an estimate and
+// redoes the batch through the maps when the total passes it.
+constexpr int EM_STREAM = 3, EM_BUILD = 4;   // columns per side (a fourth stream column spills)
+struct EmitCols {
+  int32_t ns, nb, pw;                  // stream columns, build columns, payload bytes per build row (0, 8 or 16)
+  int8_t s_w[EM_STREAM];
+  int8_t b_w[EM_BUILD], b_off[EM_BUILD];   // width and byte offset in the payload row
+  const void* s_in[EM_STREAM];         // nullptr: the join key
+  void* s_out[EM_STREAM];
+  void* b_out[EM_BUILD];
+  const void* packed;
+  unsigned long long cap;              // rows allocated in every output column
+};
+struct NoEmit {};
+
+// Columns of 4, 8 (and, on the build side, 16) bytes only: every further width is one more branch per column, and those
+// branches cost the emitting kernel registers it does not have under __launch_bounds__(SF_NT, FP_CTAS) (it spilled)
+__host__ __device__ __forceinline__ bool emit_width_ok(int w, bool build) { return w == 4 || w == 8 || (build && w == 16); }
+// every load first, then the stores: the loads are independent random accesses, and the stores could alias them
+__device__ __forceinline__ void emit_row(const EmitCols& em, uint32_t o, int32_t src, uint64_t kb, int32_t br) {   // o < cap < 2^31
+  uint64_t v[EM_STREAM];
+#pragma unroll
+  for (int c = 0; c < EM_STREAM; c++) {
+    v[c] = kb;
+    if (c < em.ns && em.s_in[c])
+      v[c] = em.s_w[c] == 8 ? __ldg(reinterpret_cast<const unsigned long long*>(em.s_in[c]) + src) : __ldg(reinterpret_cast<const uint32_t*>(em.s_in[c]) + src);
+  }
+  uint64_t lo = 0, hi = 0;
+  if (em.pw == 16) { const ulonglong2 b = __ldg(reinterpret_cast<const ulonglong2*>(em.packed) + br); lo = b.x; hi = b.y; }
+  else if (em.pw == 8) lo = __ldg(reinterpret_cast<const unsigned long long*>(em.packed) + br);
+#pragma unroll
+  for (int c = 0; c < EM_STREAM; c++) {
+    if (c >= em.ns) break;
+    if (em.s_w[c] == 8) reinterpret_cast<unsigned long long*>(em.s_out[c])[o] = v[c];
+    else reinterpret_cast<uint32_t*>(em.s_out[c])[o] = (uint32_t)v[c];
+  }
+#pragma unroll
+  for (int c = 0; c < EM_BUILD; c++) {
+    if (c >= em.nb) break;
+    const int off = em.b_off[c];
+    const uint64_t x = off & 8 ? hi : lo;
+    if (em.b_w[c] == 16) reinterpret_cast<ulonglong2*>(em.b_out[c])[o] = make_ulonglong2(lo, hi);
+    else if (em.b_w[c] == 8) reinterpret_cast<unsigned long long*>(em.b_out[c])[o] = x;
+    else reinterpret_cast<uint32_t*>(em.b_out[c])[o] = off & 4 ? (uint32_t)(x >> 32) : (uint32_t)x;
+  }
+}
+
+template <typename K, bool TRACK, bool EMIT = false>
 __device__ __forceinline__ void probe_distinct1_rows(const K* __restrict__ keys, const int32_t (&r)[PQ], const uint64_t* __restrict__ slots,
                                                      uint32_t mask, const unsigned long long* __restrict__ bloom, uint32_t bloom_mask,
                                                      unsigned long long* __restrict__ total, int32_t* __restrict__ left_map,
-                                                     int32_t* __restrict__ right_map, int32_t* s_q, uint32_t* __restrict__ track) {
+                                                     int32_t* __restrict__ right_map, int32_t* s_q, uint32_t* __restrict__ track,
+                                                     const EmitCols* em = nullptr) {
   typedef typename std::make_unsigned<K>::type UK;
   const int lane = threadIdx.x & 31;
   const uint32_t lt = (1u << lane) - 1u;
@@ -283,11 +336,13 @@ __device__ __forceinline__ void probe_distinct1_rows(const K* __restrict__ keys,
   for (int q0 = 0; q0 < qn; q0 += 32) {
     const int q = q0 + lane;
     int32_t br = INT32_MIN, src = 0;
+    uint64_t key = 0;   // EMIT: the key column's value
     if (q < qn) {
       src = s_q[q];
       const uint64_t kb = (uint64_t)(UK)keys[src];
       const uint32_t hh = hash_packed(kb);
       uint32_t idx = hh & mask;
+      key = kb;
       while (true) {
         const ulonglong2 e = *reinterpret_cast<const ulonglong2*>(&slots[(size_t)idx << 1]);
         if (e.x == JSLOT_EMPTY) break;
@@ -301,7 +356,9 @@ __device__ __forceinline__ void probe_distinct1_rows(const K* __restrict__ keys,
       unsigned long long o = 0;
       if (lane == 0) o = atomicAdd(total, (unsigned long long)__popc(b));
       o = __shfl_sync(0xffffffffu, o, 0) + __popc(b & lt);
-      if (hit) {
+      if constexpr (EMIT) {
+        if (hit && o < em->cap) emit_row(*em, (uint32_t)o, src, key, br);
+      } else if (hit) {
         left_map[o] = src; right_map[o] = br;
         if constexpr (TRACK) track_hit(track, br);
       }
@@ -345,21 +402,26 @@ __global__ void __launch_bounds__(256) join_probe_distinct1_kernel(const K* __re
 // 3 measured slower, 5 spills).
 constexpr int FP_TILE = 8 * 1024, FP_WORDS = FP_TILE / 32, FP_CTAS = 4;
 static_assert(FP_WORDS == SF_NT, "one mask word per thread");
-template <typename K, bool TRACK>
+// EMIT: the output rows are written (EmitCols `em`) instead of the maps, which are then null
+template <typename K, bool TRACK, bool EMIT = false>
 __global__ void __launch_bounds__(SF_NT, FP_CTAS) join_filter_probe_kernel(const __grid_constant__ SimplePred sp, const K* __restrict__ keys, int64_t n,
                                                                           const uint64_t* __restrict__ slots, uint32_t mask,
                                                                           const unsigned long long* __restrict__ bloom, uint32_t bloom_mask,
                                                                           unsigned long long* __restrict__ total, int32_t* __restrict__ left_map,
                                                                           int32_t* __restrict__ right_map, unsigned long long* __restrict__ npass,
-                                                                          uint32_t* __restrict__ track) {
+                                                                          uint32_t* __restrict__ track,
+                                                                          const __grid_constant__ typename std::conditional<EMIT, EmitCols, NoEmit>::type em) {
   __shared__ uint32_t s_mask[FP_WORDS];
   __shared__ uint16_t s_rows[FP_TILE];               // offsets in the tile of the passing rows, ascending
   __shared__ int32_t s_q[SF_NT / 32][32 * PQ];
   __shared__ uint32_t s_wtot[SF_NT / 32];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const int64_t ntiles = (n + FP_TILE - 1) / FP_TILE;
-  for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-    const int64_t row0 = tile * FP_TILE;
+  // a 32-bit tile index in the emitting variant (n < 2^31): the 64-bit one is the register it would otherwise spill; the maps
+  // variants keep theirs, and with it their code
+  typedef typename std::conditional<EMIT, int32_t, int64_t>::type TileIdx;
+  for (TileIdx tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    const int64_t row0 = (int64_t)tile * FP_TILE;
     sf_tile(sp, row0, (int)min((int64_t)FP_TILE, n - row0), s_mask, FP_WORDS);
     const uint32_t m = s_mask[threadIdx.x], c = __popc(m);
     uint32_t inc = c;
@@ -380,7 +442,8 @@ __global__ void __launch_bounds__(SF_NT, FP_CTAS) join_filter_probe_kernel(const
         const int q = q0 + j * 32 + lane;
         r[j] = q < qn ? (int32_t)(row0 + s_rows[q]) : -1;
       }
-      probe_distinct1_rows<K, TRACK>(keys, r, slots, mask, bloom, bloom_mask, total, left_map, right_map, s_q[w], track);
+      if constexpr (EMIT) probe_distinct1_rows<K, TRACK, true>(keys, r, slots, mask, bloom, bloom_mask, total, left_map, right_map, s_q[w], track, &em);
+      else probe_distinct1_rows<K, TRACK>(keys, r, slots, mask, bloom, bloom_mask, total, left_map, right_map, s_q[w], track);
     }
     __syncthreads();   // s_mask, s_rows and s_wtot are rewritten by the next tile
   }
@@ -605,9 +668,21 @@ static JoinTracker* tracker_from(b2_handle h) {
 // maps carry ORIGINAL row ids of `batch`, `npass_out` = rows that passed the filter (the filter node's numOutputRows).
 // tracker != 0: the build rows found are marked in it (join_filter_probe_kernel's tracking variant).
 // false = not applicable, the caller takes the selection-vector path (b2_filter_row_ids + b2_join_probe_sel).
+// whether join_filter_probe_kernel can probe `batch` with `prog` below it: the key column in `pc`, the predicate in `sp`
+static bool filter_probe_applies(const JoinTable* jt, const Table* batch, int key_col, const Program* prog, const Column*& pc, SimplePred& sp) {
+  if (getenv("B2_JOIN_NO_FAST_PROBE")) return false;
+  const int64_t n = batch->rows;
+  if (!jt->distinct || !jt->fast || jt->key_idx.size() != 1 || n < (1 << 16) || n >= 0x7fffffffLL) return false;
+  if (key_col < 0 || key_col >= (int)batch->cols.size()) throw Error(B2_ERR_INVALID, "join key index out of range");
+  pc = batch->cols[key_col];
+  const int pw = dtype_width(pc->dtype);
+  if (pc->nullable() || is_float(pc->dtype) || pc->dtype == B2_STRING || !(pw == 4 || pw == 8)) return false;
+  if (pc->dtype != jt->keys->cols[jt->key_idx[0]]->dtype) return false;
+  return simple_pred_of(prog, batch, sp);   // also: every predicate column 16-byte aligned
+}
+
 bool join_probe_pred(b2_handle ht, const Table* batch, int key_col, const Program* prog, Column** out_lm, Column** out_rm, int64_t* npass_out,
                      b2_handle tracker) {
-  if (getenv("B2_JOIN_NO_FAST_PROBE")) return false;
   JoinTable* jt = jt_from(ht);
   uint32_t* track = nullptr;
   if (tracker) {
@@ -616,14 +691,10 @@ bool join_probe_pred(b2_handle ht, const Table* batch, int key_col, const Progra
     track = tr->bits.as<uint32_t>();
   }
   const int64_t n = batch->rows;
-  if (!jt->distinct || !jt->fast || jt->key_idx.size() != 1 || n < (1 << 16) || n >= 0x7fffffffLL) return false;
-  if (key_col < 0 || key_col >= (int)batch->cols.size()) throw Error(B2_ERR_INVALID, "join key index out of range");
-  const Column* pc = batch->cols[key_col];
-  const int pw = dtype_width(pc->dtype);
-  if (pc->nullable() || is_float(pc->dtype) || pc->dtype == B2_STRING || !(pw == 4 || pw == 8)) return false;
-  if (pc->dtype != jt->keys->cols[jt->key_idx[0]]->dtype) return false;
+  const Column* pc = nullptr;
   SimplePred sp;
-  if (!simple_pred_of(prog, batch, sp)) return false;   // also: every predicate column 16-byte aligned
+  if (!filter_probe_applies(jt, batch, key_col, prog, pc, sp)) return false;
+  const int pw = dtype_width(pc->dtype);
   ColGuard lm(new_column(B2_INT32, 0, n, false)), rm(new_column(B2_INT32, 0, n, false));
   DevBuf tot(16);
   CUDA_CHECK(cudaMemsetAsync(tot.p, 0, 16, stream()));
@@ -633,17 +704,18 @@ bool join_probe_pred(b2_handle ht, const Table* batch, int key_col, const Progra
     const unsigned long long* bl = jt->bloom.as<unsigned long long>();
     unsigned long long* tp = tot.as<unsigned long long>();
     int32_t* lp = lm.c->data.as<int32_t>(); int32_t* rp = rm.c->data.as<int32_t>();
+    const NoEmit ne;
     if (track) {
       if (pw == 8) launch("join_filter_probe_track_kernel", join_filter_probe_kernel<int64_t, true>, grid, SF_NT, 0, stream(), sp, pc->data.as<int64_t>(), n,
-                          sl, msk, bl, jt->bloom_mask, tp, lp, rp, tp + 1, track);
+                          sl, msk, bl, jt->bloom_mask, tp, lp, rp, tp + 1, track, ne);
       else launch("join_filter_probe_track_kernel", join_filter_probe_kernel<int32_t, true>, grid, SF_NT, 0, stream(), sp, pc->data.as<int32_t>(), n, sl,
-                  msk, bl, jt->bloom_mask, tp, lp, rp, tp + 1, track);
+                  msk, bl, jt->bloom_mask, tp, lp, rp, tp + 1, track, ne);
     } else if (pw == 8) {
       launch("join_filter_probe_kernel", join_filter_probe_kernel<int64_t, false>, grid, SF_NT, 0, stream(), sp, pc->data.as<int64_t>(), n, sl, msk, bl,
-             jt->bloom_mask, tp, lp, rp, tp + 1, nullptr);
+             jt->bloom_mask, tp, lp, rp, tp + 1, nullptr, ne);
     } else {
       launch("join_filter_probe_kernel", join_filter_probe_kernel<int32_t, false>, grid, SF_NT, 0, stream(), sp, pc->data.as<int32_t>(), n, sl, msk, bl,
-             jt->bloom_mask, tp, lp, rp, tp + 1, nullptr);
+             jt->bloom_mask, tp, lp, rp, tp + 1, nullptr, ne);
     }
   }
   unsigned long long h[2] = {0, 0};
@@ -652,6 +724,111 @@ bool join_probe_pred(b2_handle ht, const Table* batch, int key_col, const Progra
   lm.c->size = (int64_t)h[0]; rm.c->size = (int64_t)h[0];
   *npass_out = (int64_t)h[1];
   *out_lm = lm.release(); *out_rm = rm.release();
+  return true;
+}
+
+// ---- the emitting probe's build payload: the build columns packed row-major, widest first so that every column sits at an
+// offset that is a multiple of its width and none crosses an 8-byte word (a 16-byte column fills the row) -------------------
+struct PackCols {
+  int32_t n, words;
+  int8_t w[EM_BUILD], off[EM_BUILD];
+  const void* in[EM_BUILD];
+};
+__global__ void __launch_bounds__(256) join_pack_payload_kernel(const __grid_constant__ PackCols pc, int64_t rows, unsigned long long* __restrict__ out) {
+  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < rows; r += (int64_t)gridDim.x * blockDim.x) {
+    uint64_t lo = 0, hi = 0;
+    for (int c = 0; c < pc.n; c++) {
+      if (pc.w[c] == 16) { const ulonglong2 v = reinterpret_cast<const ulonglong2*>(pc.in[c])[r]; lo = v.x; hi = v.y; continue; }
+      const uint64_t v = (pc.w[c] == 8 ? reinterpret_cast<const unsigned long long*>(pc.in[c])[r] : (uint64_t)reinterpret_cast<const uint32_t*>(pc.in[c])[r])
+                         << (8 * (pc.off[c] & 7));
+      if (pc.off[c] & 8) hi |= v; else lo |= v;
+    }
+    if (pc.words == 2) reinterpret_cast<ulonglong2*>(out)[r] = make_ulonglong2(lo, hi);
+    else out[r] = lo;
+  }
+}
+
+bool join_pack_payload(const Table* build, const std::vector<int>& cols, JoinPayload& pl) {
+  if (cols.size() > (size_t)EM_BUILD) return false;
+  int bytes = 0;
+  for (int c : cols) {
+    if (c < 0 || c >= (int)build->cols.size()) throw Error(B2_ERR_INVALID, "join column index out of range");
+    const Column* bc = build->cols[c];
+    if (bc->nullable() || bc->dtype == B2_STRING || !emit_width_ok(dtype_width(bc->dtype), true)) return false;
+    bytes += dtype_width(bc->dtype);
+  }
+  if (bytes > 16) return false;
+  pl.width = bytes == 0 ? 0 : (bytes <= 8 ? 8 : 16);
+  pl.dtype.clear(); pl.scale.clear(); pl.off.assign(cols.size(), 0);
+  for (int c : cols) { pl.dtype.push_back(build->cols[c]->dtype); pl.scale.push_back(build->cols[c]->scale); }
+  PackCols pc; memset(&pc, 0, sizeof(pc));
+  pc.words = pl.width / 8;
+  int at = 0;
+  for (int w = 16; w >= 4; w >>= 1)
+    for (size_t k = 0; k < cols.size(); k++) {
+      if (dtype_width(pl.dtype[k]) != w) continue;
+      pl.off[k] = at;
+      pc.w[pc.n] = (int8_t)w; pc.off[pc.n] = (int8_t)at; pc.in[pc.n] = build->cols[cols[k]]->data.p; pc.n++;
+      at += w;
+    }
+  const int64_t rows = build->rows;
+  pl.packed = DevBuf(pl.width ? (size_t)rows * pl.width : 0);
+  if (pl.width && rows)
+    launch("join_pack_payload_kernel", join_pack_payload_kernel, grid_for(rows, 256), 256, 0, stream(), pc, rows, pl.packed.as<unsigned long long>());
+  return true;
+}
+
+bool join_probe_pred_emit(b2_handle ht, const Table* batch, int key_col, const Program* prog, const std::vector<int>& stream_cols,
+                          const JoinPayload& pl, int64_t cap, Table** out, int64_t* total_out, int64_t* npass_out) {
+  JoinTable* jt = jt_from(ht);
+  const Column* pc = nullptr;
+  SimplePred sp;
+  if (!filter_probe_applies(jt, batch, key_col, prog, pc, sp) || stream_cols.size() > (size_t)EM_STREAM) return false;
+  if (pl.packed.bytes != (size_t)jt->build_rows * pl.width) throw Error(B2_ERR_INVALID, "join payload does not match the hash table");
+  for (int c : stream_cols) {
+    if (c < 0 || c >= (int)batch->cols.size()) throw Error(B2_ERR_INVALID, "join column index out of range");
+    const Column* ic = batch->cols[c];
+    if (ic->nullable() || ic->dtype == B2_STRING || !emit_width_ok(dtype_width(ic->dtype), false)) return false;
+  }
+  EmitCols em; memset(&em, 0, sizeof(em));
+  ColsGuard outs;
+  for (int c : stream_cols) {
+    const Column* ic = batch->cols[c];
+    outs.v.push_back(new_column(ic->dtype, ic->scale, cap, false));
+    em.s_w[em.ns] = (int8_t)dtype_width(ic->dtype);
+    em.s_in[em.ns] = c == key_col ? nullptr : ic->data.p;
+    em.s_out[em.ns++] = outs.v.back()->data.p;
+  }
+  for (size_t k = 0; k < pl.dtype.size(); k++) {
+    outs.v.push_back(new_column(pl.dtype[k], pl.scale[k], cap, false));
+    em.b_w[em.nb] = (int8_t)dtype_width(pl.dtype[k]); em.b_off[em.nb] = (int8_t)pl.off[k];
+    em.b_out[em.nb++] = outs.v.back()->data.p;
+  }
+  em.pw = pl.width; em.packed = pl.packed.p; em.cap = (unsigned long long)cap;
+  const int64_t n = batch->rows;
+  DevBuf tot(16);
+  CUDA_CHECK(cudaMemsetAsync(tot.p, 0, 16, stream()));
+  {
+    const int grid = grid_for(n, FP_TILE, FP_CTAS);
+    const uint64_t* sl = jt->slots.as<uint64_t>(); const uint32_t msk = (uint32_t)(jt->cap - 1);
+    const unsigned long long* bl = jt->bloom.as<unsigned long long>();
+    unsigned long long* tp = tot.as<unsigned long long>();
+    if (dtype_width(pc->dtype) == 8)
+      launch("join_filter_probe_kernel", join_filter_probe_kernel<int64_t, false, true>, grid, SF_NT, 0, stream(), sp, pc->data.as<int64_t>(), n, sl, msk,
+             bl, jt->bloom_mask, tp, nullptr, nullptr, tp + 1, nullptr, em);
+    else
+      launch("join_filter_probe_kernel", join_filter_probe_kernel<int32_t, false, true>, grid, SF_NT, 0, stream(), sp, pc->data.as<int32_t>(), n, sl, msk,
+             bl, jt->bloom_mask, tp, nullptr, nullptr, tp + 1, nullptr, em);
+  }
+  unsigned long long h[2] = {0, 0};
+  d2h(h, tot.p, 2);
+  sync();
+  *total_out = (int64_t)h[0];
+  *npass_out = (int64_t)h[1];
+  if ((int64_t)h[0] <= cap) {
+    for (Column* c : outs.v) c->size = (int64_t)h[0];
+    *out = new_table(outs.release());
+  }
   return true;
 }
 

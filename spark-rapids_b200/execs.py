@@ -56,6 +56,14 @@ class HashJoinExec(GpuExec):
         check(lib.b2_exec_join_sub_partition_stats(self.h, out))
         return {"buckets": out[0], "repartitioned": out[1], "build_bytes": out[2], "stream_bytes": out[3]}
 
+    @property
+    def emit_stats(self):
+        """stream batches whose output rows the filter-probe kernel wrote, batches joined through gather maps, and
+        overflow reruns (emitted batches whose matches passed the estimated output size, joined again through the maps)"""
+        out = (ctypes.c_int64 * 3)()
+        check(lib.b2_exec_join_emit_stats(self.h, out))
+        return {"emitted": out[0], "maps": out[1], "overflows": out[2]}
+
 
 def _new(fn, *args, keep=(), cls=GpuExec):
     out = ctypes.c_int64()
