@@ -417,6 +417,39 @@ int b2_comm_stats(b2_handle comm, int64_t* out4);
 /* GpuBroadcastExchangeExec data movement: root's table to every rank (ncclBroadcast); non-root pass table = 0 */
 int b2_broadcast_table(b2_handle comm, b2_handle table, int32_t root, b2_handle* out_table);
 
+/* ---- a13: window (GpuWindowExec.scala, GpuRunningWindowExec.scala, GpuWindowExpression.scala; BasicWindowCalc.scala:435-521)
+ * The input is sorted by (partition keys, order keys).  A partition is a maximal run of adjacent rows with equal partition keys,
+ * a peer group a run inside it with equal order keys too; "equal" is the sort's normalised key (NULL = NULL, NaN = NaN,
+ * -0.0 = 0.0, strings byte for byte).  Unsorted input is not checked: each contiguous run is a partition.
+ *   ROW_NUMBER / RANK / DENSE_RANK -> INT32; LEAD / LAG -> the column's type, the default where i +- offset leaves the partition
+ *   (a NULL value at a row that exists stays NULL; a non-NULL default on STRING: B2_ERR_UNSUPPORTED).  All five need ORDER BY.
+ *   SUM: integers -> INT64 (wraps), floats -> FLOAT64, DECIMAL(p, s) -> out_dtype DECIMAL(out_precision, s) computed exactly: a
+ *   running frame is NULL from the first row whose running value does not fit on, to the partition's end (SumBinaryFixer); other
+ *   frames are NULL when the frame's total does not fit.  COUNT / COUNT_ALL -> INT64 (0 on an empty frame).  MIN / MAX -> the
+ *   column's type, b2_groupby's order (NaN greatest); STRING and DECIMAL128: B2_ERR_UNSUPPORTED.  SUM, MIN, MAX are NULL on an
+ *   empty or all-NULL frame.  Frames: ROWS [lower, upper] (row offsets, 0 = CURRENT ROW, or the UNBOUNDED sentinels, clipped to
+ *   the partition); RANGE only UNBOUNDED PRECEDING -> CURRENT ROW (to the end of the peer group) or -> UNBOUNDED FOLLOWING
+ *   (value offsets: B2_ERR_UNSUPPORTED).  A float SUM is a parallel scan: it may differ from a left-to-right sum in the last bits. */
+typedef enum {
+  B2_WIN_ROW_NUMBER = 1, B2_WIN_RANK = 2, B2_WIN_DENSE_RANK = 3, B2_WIN_LEAD = 4, B2_WIN_LAG = 5,
+  B2_WIN_SUM = 10, B2_WIN_COUNT = 11, B2_WIN_COUNT_ALL = 12, B2_WIN_MIN = 13, B2_WIN_MAX = 14
+} b2_window_kind;
+typedef enum { B2_FRAME_ROWS = 0, B2_FRAME_RANGE = 1 } b2_frame_type;
+#define B2_UNBOUNDED_PRECEDING INT64_MIN
+#define B2_UNBOUNDED_FOLLOWING INT64_MAX
+typedef struct {
+  int32_t kind, column;            /* column ignored by ROW_NUMBER / RANK / DENSE_RANK / COUNT_ALL */
+  int32_t frame;                   /* b2_frame_type; ignored by the ranking functions and LEAD / LAG */
+  int32_t offset;                  /* LEAD / LAG, >= 0 */
+  int64_t lower, upper;            /* frame bounds */
+  uint8_t default_value[16];       /* LEAD / LAG default, b2_expr_literal's encoding */
+  int32_t default_is_null;
+  int32_t out_dtype, out_precision, out_scale;   /* read by decimal SUM only (DECIMAL64 or DECIMAL128; scale = the input's) */
+} b2_window_spec;
+/* one sorted batch: output = the input columns, then one column per spec */
+int b2_window(b2_handle table, const int32_t* part_cols, int32_t nparts, const b2_order_by_arg* order, int32_t norder,
+              const b2_window_spec* specs, int32_t nspecs, b2_handle* out_table);
+
 /* ---- host operator layer: C++ mirror of the GpuExec nodes of the hot path (exec.cu).  Every node is
  * a pull iterator of batches — GpuExec.internalDoExecuteColumnar(): RDD[ColumnarBatch]
  * (GpuExec.scala:106,190,380).  b2_exec_next returns 0 in *out_table when the node is exhausted. */
@@ -498,6 +531,13 @@ int b2_exec_broadcast_exchange(b2_handle child, b2_handle comm, int32_t rank, in
 /* GpuSortExec (global != 0: full sort, else each batch) / GpuTopN when limit >= 0 */
 int b2_exec_sort(b2_handle child, const b2_order_by_arg* order, int32_t norder, int32_t global, int64_t limit, b2_handle* out);
 int b2_exec_coalesce(b2_handle child, int64_t target_rows, b2_handle* out);                    /* GpuCoalesceBatches */
+/* GpuWindowExec / GpuRunningWindowExec (GpuWindowExec.scala:145-161, GpuRunningWindowExec.scala:42-250): b2_window over a child
+ * sorted by (part_cols, order), e.g. by GpuSortExec.  Only running frames and ranking: one output batch per non-empty input batch,
+ * continued across batches on the device (an allocation failure halves a batch: each half becomes an output batch).  A RANGE running frame: each batch's trailing peer group waits for the next batch.  A
+ * whole-partition or bounded frame, or LEAD / LAG: the trailing partition waits (no PARTITION BY: the whole input is one batch).
+ * Waiting rows are held in the spill store; a group of 2^31-1 rows or more: B2_ERR_SIZE_OVERFLOW. */
+int b2_exec_window(b2_handle child, const int32_t* part_cols, int32_t nparts, const b2_order_by_arg* order, int32_t norder,
+                   const b2_window_spec* specs, int32_t nspecs, b2_handle* out);
 /* GpuShuffleExchangeExec: hash partition on key_cols (none = SinglePartition) + NCCL all-to-all */
 int b2_exec_shuffle_exchange(b2_handle child, const int32_t* key_cols, int32_t nkeys, b2_handle comm, int32_t world, b2_handle* out);
 int b2_exec_next(b2_handle exec, b2_handle* out_table);

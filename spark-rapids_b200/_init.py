@@ -6,7 +6,7 @@ implementation here: every operation goes to the library, which fails loudly wit
 import ctypes
 import numpy as np
 
-from ._lib import lib, check, B2Error, B2ColumnInfo, B2AggSpec, B2OrderByArg, B2HostColumn, parse_header, LIB_PATH  # noqa: F401
+from ._lib import lib, check, B2Error, B2ColumnInfo, B2AggSpec, B2OrderByArg, B2HostColumn, B2WindowSpec, parse_header, LIB_PATH  # noqa: F401
 
 # b2_dtype
 BOOL8, INT8, INT16, INT32, INT64, FLOAT32, FLOAT64, DATE32, TIMESTAMP_US, DECIMAL32, DECIMAL64, DECIMAL128, STRING = range(13)
@@ -24,6 +24,11 @@ OP_NORMALIZE_NAN_ZERO, OP_YEAR = 41, 42
 OP_STARTS_WITH, OP_ENDS_WITH, OP_CONTAINS, OP_LIKE, OP_SUBSTRING = 50, 51, 52, 53, 54
 # b2_agg_kind
 AGG_SUM, AGG_COUNT, AGG_MIN, AGG_MAX, AGG_COUNT_ALL = 1, 2, 3, 4, 5
+# b2_window_kind, b2_frame_type
+WIN_ROW_NUMBER, WIN_RANK, WIN_DENSE_RANK, WIN_LEAD, WIN_LAG = 1, 2, 3, 4, 5
+WIN_SUM, WIN_COUNT, WIN_COUNT_ALL, WIN_MIN, WIN_MAX = 10, 11, 12, 13, 14
+FRAME_ROWS, FRAME_RANGE = 0, 1
+UNBOUNDED_PRECEDING, UNBOUNDED_FOLLOWING = -2**63, 2**63 - 1
 # b2_join_kind
 JOIN_INNER, JOIN_LEFT_OUTER, JOIN_LEFT_SEMI, JOIN_LEFT_ANTI, JOIN_FULL_OUTER, JOIN_RIGHT_OUTER = 0, 1, 2, 3, 4, 5
 
@@ -407,6 +412,127 @@ def _order_args(keys):
     for i, k in enumerate(keys):
         arr[i].column, arr[i].ascending, arr[i].nulls_first = int(k[0]), int(k[1]), int(k[2])
     return arr
+
+
+class Frame:
+    """a window frame: ROWS or RANGE, bounds as row offsets (0 = CURRENT ROW, None = UNBOUNDED)"""
+
+    def __init__(self, frame_type, lower, upper):
+        self.type, self.lower, self.upper = frame_type, lower, upper
+
+
+def rows(lower, upper):
+    """ROWS BETWEEN lower AND upper (None = UNBOUNDED PRECEDING / FOLLOWING)"""
+    return Frame(FRAME_ROWS, lower, upper)
+
+
+def range_running():
+    """RANGE BETWEEN UNBOUNDED PRECEDING AND CURRENT ROW: Spark's default frame with ORDER BY"""
+    return Frame(FRAME_RANGE, None, 0)
+
+
+def unbounded():
+    """the whole partition: Spark's default frame without ORDER BY"""
+    return Frame(FRAME_ROWS, None, None)
+
+
+class WindowFunc:
+    """one window function: kind (WIN_*), its column, a Frame (aggregates), LEAD / LAG offset and default, and for a decimal
+    SUM the result type (out_dtype, out_precision; the scale is the input's)"""
+
+    def __init__(self, kind, column=0, frame=None, offset=1, default=None, default_dtype=None, out_dtype=0, out_precision=0):
+        self.kind, self.column, self.frame, self.offset = kind, column, frame, offset
+        self.default, self.default_dtype = default, default_dtype
+        self.out_dtype, self.out_precision = out_dtype, out_precision
+
+
+def row_number():
+    return WindowFunc(WIN_ROW_NUMBER)
+
+
+def rank():
+    return WindowFunc(WIN_RANK)
+
+
+def dense_rank():
+    return WindowFunc(WIN_DENSE_RANK)
+
+
+def _offset_default(default, dtype):
+    if isinstance(default, float) and dtype not in (FLOAT32, FLOAT64):
+        raise ValueError("a float LEAD / LAG default needs dtype=FLOAT32 or FLOAT64 (the column's type)")
+    return default
+
+
+def lead(column, offset=1, default=None, dtype=None):
+    """dtype: the column's type, required with a float default (FLOAT32 and FLOAT64 defaults are encoded differently)"""
+    return WindowFunc(WIN_LEAD, column, offset=offset, default=_offset_default(default, dtype), default_dtype=dtype)
+
+
+def lag(column, offset=1, default=None, dtype=None):
+    return WindowFunc(WIN_LAG, column, offset=offset, default=_offset_default(default, dtype), default_dtype=dtype)
+
+
+def win_sum(column, frame, out_dtype=0, out_precision=0):
+    """decimal columns: out_dtype DECIMAL64 / DECIMAL128 and out_precision (Spark: min(38, p + 10))"""
+    return WindowFunc(WIN_SUM, column, frame, out_dtype=out_dtype, out_precision=out_precision)
+
+
+def win_count(column, frame):
+    return WindowFunc(WIN_COUNT, column, frame)
+
+
+def win_count_all(frame):
+    return WindowFunc(WIN_COUNT_ALL, 0, frame)
+
+
+def win_min(column, frame):
+    return WindowFunc(WIN_MIN, column, frame)
+
+
+def win_max(column, frame):
+    return WindowFunc(WIN_MAX, column, frame)
+
+
+def _literal16(value, dtype):
+    buf = np.zeros(2, dtype=np.uint64)
+    if dtype == FLOAT32:
+        buf[0] = int(np.array([value], dtype=np.float32).view(np.uint32)[0])
+    elif dtype == FLOAT64:
+        buf[0] = np.array([value], dtype=np.float64).view(np.uint64)[0]
+    else:
+        v = int(value) & ((1 << 128) - 1)
+        buf[0] = v & 0xFFFFFFFFFFFFFFFF
+        buf[1] = v >> 64
+    return buf.view(np.uint8)
+
+
+def _window_specs(funcs):
+    """funcs: WindowFunc objects, or tuples (kind, column, frame, ...) of WindowFunc's arguments"""
+    arr = (B2WindowSpec * max(len(funcs), 1))()
+    for i, f in enumerate(funcs):
+        if not isinstance(f, WindowFunc):
+            f = WindowFunc(*f)
+        s = arr[i]
+        s.kind, s.column, s.offset = f.kind, f.column, f.offset
+        fr = f.frame or Frame(FRAME_ROWS, None, 0)
+        s.frame = fr.type
+        s.lower = UNBOUNDED_PRECEDING if fr.lower is None else fr.lower
+        s.upper = UNBOUNDED_FOLLOWING if fr.upper is None else fr.upper
+        s.default_is_null = int(f.default is None)
+        if f.default is not None:
+            s.default_value[:] = list(_literal16(f.default, f.default_dtype))
+        s.out_dtype, s.out_precision = f.out_dtype, f.out_precision
+    return arr
+
+
+def window(table, partition_by, order_by, funcs):
+    """b2_window over one batch sorted by (partition_by, order_by): the input columns, then one column per function.
+    order_by: (column, ascending, nulls_first) tuples"""
+    out = ctypes.c_int64()
+    check(lib.b2_window(table.h, _i32s(partition_by), len(partition_by), _order_args(order_by), len(order_by), _window_specs(funcs), len(funcs),
+                        ctypes.byref(out)))
+    return Table(out.value)
 
 
 def init(device=0, pool_bytes=0):

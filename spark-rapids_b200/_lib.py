@@ -35,6 +35,13 @@ class B2OrderByArg(ctypes.Structure):
     _fields_ = [("column", ctypes.c_int32), ("ascending", ctypes.c_int32), ("nulls_first", ctypes.c_int32)]
 
 
+class B2WindowSpec(ctypes.Structure):
+    _fields_ = [("kind", ctypes.c_int32), ("column", ctypes.c_int32), ("frame", ctypes.c_int32), ("offset", ctypes.c_int32),
+                ("lower", ctypes.c_int64), ("upper", ctypes.c_int64), ("default_value", ctypes.c_uint8 * 16),
+                ("default_is_null", ctypes.c_int32), ("out_dtype", ctypes.c_int32), ("out_precision", ctypes.c_int32),
+                ("out_scale", ctypes.c_int32)]
+
+
 def _arg_type(decl):
     decl = decl.strip()
     if "*" in decl:

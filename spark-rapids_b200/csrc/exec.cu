@@ -16,12 +16,14 @@
 //   GpuSortExec / GpuTopN     GpuSortExec.scala:87-165 (each-batch | full), limit.scala:234-330
 //   GpuCoalesceBatches        GpuCoalesceBatches.scala:160-239 (TargetSize goal by rows)
 //   GpuShuffleExchangeExec    GpuShuffleExchangeExecBase.scala:384-536 with the NCCL all-to-all
+//   GpuWindowExec             GpuWindowExec.scala:145-161 + GpuRunningWindowExec.scala:42-250 (window.cu)
 #include <algorithm>
 #include <chrono>
 #include <cmath>
 #include <deque>
 #include "joinemit.cuh"
 #include "vm.cuh"
+#include "window.cuh"
 
 namespace b2 {
 
@@ -1400,6 +1402,89 @@ struct GpuOutOfCoreSortExec : GpuExec {
   }
 };
 
+// GpuWindowExec / GpuRunningWindowExec (GpuWindowExec.scala:145-161, GpuRunningWindowExec.scala:42-250) over a child sorted by
+// (partition, order).  The batching follows the most demanding function:
+//   1. running frames and ranking only: every batch on its own, continuing from the carry of the one before (the last row and
+//      each function's state, on the device); an OOM splits the batch in halves, which the carry makes equivalent;
+//   2. a RANGE running frame: the trailing peer group of each batch waits for the next (BatchedByKey(partition ++ order));
+//   3. a whole-partition or bounded frame, or LEAD / LAG: the trailing partition waits (BatchedByKey(partition); with no
+//      PARTITION BY the whole input is one group, RequireSingleBatch).
+// Waiting rows are pieces in the spill store, concatenated once when their group ends; finding the group end of a batch costs
+// one device-to-host copy of an index.
+struct GpuWindowExec : GpuExec {
+  WindowPlan plan;
+  WindowCarry carry;
+  bool bound = false, done = false;
+  std::deque<TableRef> pending;   // mode 1: the later pieces of a split batch, in row order, run by the next calls
+  std::vector<SpillPiece> held;   // modes 2 and 3: rows of the group still open
+  int64_t held_rows = 0;
+  TableRef held_last;             // the last held row
+
+  // mode 1: on an OOM the batch is halved; the first half runs now and the second waits in `pending` (the carry makes the halves
+  // equivalent to the whole, and each half leaves as its own output batch, so no concatenation is needed)
+  Table* run(const Table* t) {
+    try {
+      return with_retry([&] { return window_chunk(plan, t, &carry); });
+    } catch (const Error& e) {
+      if (plan.mode != 1 || !splittable(e) || t->rows < 2) throw;
+      note_split();
+      const int64_t h = t->rows / 2;
+      TableRef a(with_retry([&] { return slice_table(t, 0, h); }));
+      pending.emplace_front(with_retry([&] { return slice_table(t, h, t->rows); }));
+      return run(a.t);
+    }
+  }
+  static void hold(std::vector<SpillPiece>& into, int64_t& rows, const Table* t) {
+    if (rows + t->rows > 0x7fffffffLL) throw Error(B2_ERR_SIZE_OVERFLOW, "window: a partition of more than 2^31-1 rows");
+    SpillPiece p;
+    p.hold(t);
+    into.push_back(std::move(p));
+    rows += t->rows;
+  }
+  Table* flush(std::vector<SpillPiece>& pieces) {
+    TableRef chunk(concat_pieces(pieces, nullptr));
+    pieces.clear();
+    return run(chunk.t);
+  }
+  Table* do_next() override {
+    if (!pending.empty()) {
+      TableRef t(std::move(pending.front()));
+      pending.pop_front();
+      return run(t.t);
+    }
+    while (true) {
+      if (done) return nullptr;
+      TableRef in(children[0]->next());
+      if (!in.t) {
+        done = true;
+        held_rows = 0;
+        return held.empty() ? nullptr : flush(held);
+      }
+      if (in.t->rows == 0) continue;
+      if (!bound) { bind_window(plan, in.t); bound = true; }
+      if (plan.mode == 1) return run(in.t);
+      const int64_t n = in.t->rows;
+      const int64_t start = with_retry([&] { return window_last_start(plan, in.t, held_last.t, plan.mode == 3 ? 1 : 2); });
+      TableRef last(slice_table(in.t, n - 1, n));
+      if (start < 0) {   // the whole batch continues the open group
+        hold(held, held_rows, in.t);
+        held_last = std::move(last);
+        continue;
+      }
+      // the group that ends here runs now; the next group's first rows are already in the spill store, so that they can leave
+      // the device while it runs
+      std::vector<SpillPiece> ended = std::move(held);
+      int64_t ended_rows = held_rows;
+      held.clear();
+      held_rows = 0;
+      if (start > 0) { TableRef head(slice_table(in.t, 0, start)); hold(ended, ended_rows, head.t); }
+      { TableRef tail(slice_table(in.t, start, n)); hold(held, held_rows, tail.t); }
+      held_last = std::move(last);
+      if (!ended.empty()) return flush(ended);
+    }
+  }
+};
+
 struct GpuCoalesceBatches : GpuExec {
   int64_t target_rows = 1 << 30;
   TableRef carry;
@@ -1758,6 +1843,17 @@ int b2_exec_sort_out_of_core(b2_handle child, const b2_order_by_arg* order, int3
   *out = to_handle(e);
   B2_CATCH
 }
+int b2_exec_window(b2_handle child, const int32_t* part_cols, int32_t nparts, const b2_order_by_arg* order, int32_t norder,
+                   const b2_window_spec* specs, int32_t nspecs, b2_handle* out) {
+  B2_TRY
+  auto* e = new GpuWindowExec();
+  std::unique_ptr<GpuExec, void (*)(GpuExec*)> g(e, [](GpuExec* x) { x->release(); });
+  e->plan = make_window_plan(part_cols, nparts, order, norder, specs, nspecs);
+  e->add_child(exec_from(child));
+  *out = to_handle(g.release());
+  B2_CATCH
+}
+
 int b2_exec_coalesce(b2_handle child, int64_t target_rows, b2_handle* out) {
   B2_TRY
   auto* e = new GpuCoalesceBatches();

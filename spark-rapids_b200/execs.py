@@ -215,6 +215,13 @@ def GpuTopN(limit, sort_order, child):
     return _new(lib.b2_exec_sort, child.h, m._order_args(sort_order), len(sort_order), 1, limit, keep=[child])
 
 
+def GpuWindowExec(child, partition_by, order_by, funcs):
+    """GpuWindowExec / GpuRunningWindowExec over a child sorted by (partition_by, order_by), e.g. a GpuSortExec: the child's
+    columns, then one column per window function (spark_rapids_b200.row_number(), win_sum(col, rows(-6, 0)), ... or tuples)"""
+    return _new(lib.b2_exec_window, child.h, m._i32s(partition_by), len(partition_by), m._order_args(order_by), len(order_by),
+                m._window_specs(funcs), len(funcs), keep=[child])
+
+
 def GpuCoalesceBatches(child, target_rows):
     return _new(lib.b2_exec_coalesce, child.h, target_rows, keep=[child])
 
