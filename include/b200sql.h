@@ -531,11 +531,23 @@ int b2_exec_broadcast_exchange(b2_handle child, b2_handle comm, int32_t rank, in
 /* GpuSortExec (global != 0: full sort, else each batch) / GpuTopN when limit >= 0 */
 int b2_exec_sort(b2_handle child, const b2_order_by_arg* order, int32_t norder, int32_t global, int64_t limit, b2_handle* out);
 int b2_exec_coalesce(b2_handle child, int64_t target_rows, b2_handle* out);                    /* GpuCoalesceBatches */
-/* GpuWindowExec / GpuRunningWindowExec (GpuWindowExec.scala:145-161, GpuRunningWindowExec.scala:42-250): b2_window over a child
- * sorted by (part_cols, order), e.g. by GpuSortExec.  Only running frames and ranking: one output batch per non-empty input batch,
- * continued across batches on the device (an allocation failure halves a batch: each half becomes an output batch).  A RANGE running frame: each batch's trailing peer group waits for the next batch.  A
- * whole-partition or bounded frame, or LEAD / LAG: the trailing partition waits (no PARTITION BY: the whole input is one batch).
- * Waiting rows are held in the spill store; a group of 2^31-1 rows or more: B2_ERR_SIZE_OVERFLOW. */
+/* GpuWindowExec / GpuRunningWindowExec / GpuBatchedBoundedWindowExec (GpuWindowExec.scala:145-161, GpuRunningWindowExec.scala:
+ * 42-250, GpuBatchedBoundedWindowExec.scala): b2_window over a child sorted by (part_cols, order), e.g. by GpuSortExec.  The
+ * functions decide how it batches; the results are b2_window's over the concatenated input (a running float SUM may differ in
+ * the last bits across batch edges).
+ *   Running: only ranking and ROWS UNBOUNDED PRECEDING -> CURRENT ROW frames.  One output batch per non-empty input batch,
+ *     continued across batches by a carry on the device.  Holds one batch.
+ *   Bounded: only ranking, LEAD / LAG and ROWS frames with a finite upper bound, reaching P rows before a row and F after it
+ *     (P + F > 0).  Each batch waits in the spill store until F rows after it have arrived (or the input ends), then runs over
+ *     the columns the functions read: P + 1 rows before it, its own rows and F rows after it.  One output batch per non-empty
+ *     input batch: the batch's own columns (the same buffers) and the function columns.  Holds the waiting batches and P + 1
+ *     rows of context; neither the input nor a partition has to fit on the device, and the input may pass 2^31 rows.  A batch
+ *     plus P + F rows of 2^31 or more: B2_ERR_SIZE_OVERFLOW.
+ *   Held: any other plan.  With RANGE running frames beside running functions only, each batch's trailing peer group waits
+ *     for the next batch; otherwise (a frame to UNBOUNDED FOLLOWING, or a bounded function beside a RANGE frame) the trailing
+ *     partition waits (no PARTITION BY: the whole input is one group).  Waiting rows are held in the spill store and concatenated when their group
+ *     ends; a group of 2^31-1 rows or more: B2_ERR_SIZE_OVERFLOW.
+ * Running and bounded: an allocation failure halves a batch, and each half becomes an output batch. */
 int b2_exec_window(b2_handle child, const int32_t* part_cols, int32_t nparts, const b2_order_by_arg* order, int32_t norder,
                    const b2_window_spec* specs, int32_t nspecs, b2_handle* out);
 /* GpuShuffleExchangeExec: hash partition on key_cols (none = SinglePartition) + NCCL all-to-all */

@@ -16,7 +16,8 @@
 //   GpuSortExec / GpuTopN     GpuSortExec.scala:87-165 (each-batch | full), limit.scala:234-330
 //   GpuCoalesceBatches        GpuCoalesceBatches.scala:160-239 (TargetSize goal by rows)
 //   GpuShuffleExchangeExec    GpuShuffleExchangeExecBase.scala:384-536 with the NCCL all-to-all
-//   GpuWindowExec             GpuWindowExec.scala:145-161 + GpuRunningWindowExec.scala:42-250 (window.cu)
+//   GpuWindowExec             GpuWindowExec.scala:145-161 + GpuRunningWindowExec.scala:42-250 + GpuBatchedBoundedWindowExec.scala
+//                             (window.cu)
 #include <algorithm>
 #include <chrono>
 #include <cmath>
@@ -1406,11 +1407,17 @@ struct GpuOutOfCoreSortExec : GpuExec {
 // (partition, order).  The batching follows the most demanding function:
 //   1. running frames and ranking only: every batch on its own, continuing from the carry of the one before (the last row and
 //      each function's state, on the device); an OOM splits the batch in halves, which the carry makes equivalent;
+//   bounded: ranking, LEAD / LAG and ROWS frames with a finite upper bound, reaching P rows back and F ahead (P + F > 0;
+//      GpuBatchedBoundedWindowExec): every batch waits in the spill store until F rows after it have arrived, then runs as one
+//      chunk of the read columns only: P + 1 rows of context before it (so that no frame of its rows starts at the chunk's first
+//      row, where a difference of prefixes would need the state before the chunk), its own rows and F rows of look-ahead.  Only
+//      its own rows are written, and the output batch is its own columns (by reference) and the function columns.  The carry is
+//      taken at the row before the next chunk's first row.  An OOM splits the batch in halves, each run with its own context;
 //   2. a RANGE running frame: the trailing peer group of each batch waits for the next (BatchedByKey(partition ++ order));
-//   3. a whole-partition or bounded frame, or LEAD / LAG: the trailing partition waits (BatchedByKey(partition); with no
-//      PARTITION BY the whole input is one group, RequireSingleBatch).
-// Waiting rows are pieces in the spill store, concatenated once when their group ends; finding the group end of a batch costs
-// one device-to-host copy of an index.
+//   3. a frame to the partition's end, or a bounded frame or LEAD / LAG beside a RANGE frame: the trailing partition waits
+//      (BatchedByKey(partition); with no PARTITION BY the whole input is one group, RequireSingleBatch).
+// Waiting rows of modes 2 and 3 are pieces in the spill store, concatenated once when their group ends; finding the group end of a
+// batch costs one device-to-host copy of an index.
 struct GpuWindowExec : GpuExec {
   WindowPlan plan;
   WindowCarry carry;
@@ -1419,6 +1426,13 @@ struct GpuWindowExec : GpuExec {
   std::vector<SpillPiece> held;   // modes 2 and 3: rows of the group still open
   int64_t held_rows = 0;
   TableRef held_last;             // the last held row
+  // bounded: the plan over chunks of the read columns, the input batches waiting for their look-ahead (front first) and the
+  // context, the last P + 1 read rows before the front batch
+  WindowPlan chunk_plan;
+  std::vector<int> read_cols;
+  std::deque<SpillPiece> waiting;
+  int64_t waiting_rows = 0;
+  SpillPiece context;
 
   // mode 1: on an OOM the batch is halved; the first half runs now and the second waits in `pending` (the carry makes the halves
   // equivalent to the whole, and each half leaves as its own output batch, so no concatenation is needed)
@@ -1446,7 +1460,92 @@ struct GpuWindowExec : GpuExec {
     pieces.clear();
     return run(chunk.t);
   }
+  // the read columns of t, by reference
+  Table* read_view(const Table* t) const {
+    ColsGuard cols;
+    for (int c : read_cols) { col_incref(t->cols[c]); cols.v.push_back(t->cols[c]); }
+    return new_table(cols.release());
+  }
+  // bounded: the front batch's output, its context, rows and look-ahead in one chunk
+  Table* run_front() {
+    TableRef whole(waiting.front().get());
+    const int64_t rows = whole.t->rows, ctx = context.sp ? context.rows : 0;
+    std::vector<TableRef> parts;
+    if (ctx) parts.emplace_back(context.get());
+    parts.emplace_back(read_view(whole.t));
+    int64_t need = plan.post, total = ctx + rows;
+    for (size_t j = 1; j < waiting.size() && need > 0; j++) {
+      TableRef b(waiting[j].get());
+      TableRef v(read_view(b.t));
+      const int64_t take = std::min(need, b.t->rows);
+      parts.emplace_back(take == b.t->rows ? v.release() : with_retry([&] { return slice_table(v.t, 0, take); }));
+      need -= take;
+      total += take;
+    }
+    if (total > 0x7fffffffLL) throw Error(B2_ERR_SIZE_OVERFLOW, "window: a batch and its context and look-ahead pass 2^31-1 rows");
+    TableRef chunk;
+    if (parts.size() == 1) chunk = std::move(parts[0]);
+    else {
+      std::vector<const Table*> ts;
+      for (auto& t : parts) ts.push_back(t.t);
+      chunk = TableRef(with_retry([&] { return concat_tables(ts); }));
+    }
+    parts.clear();
+    // the next context: the last P + 1 rows up to the end of this batch; the carry is taken at the row before it
+    const int64_t keep = std::min(plan.pre + 1, ctx + rows), hi = ctx + rows;
+    SpillPiece nc;
+    {
+      TableRef next_ctx(with_retry([&] { return slice_table(chunk.t, hi - keep, hi); }));
+      nc.hold(next_ctx.t);
+    }
+    // the carry moves on only when this succeeds, and nothing after it can fail, so a retry or a split starts from a clean state
+    TableRef fns(with_retry([&] { return window_chunk_rows(chunk_plan, chunk.t, &carry, ctx, hi, hi - keep - 1); }));
+    ColsGuard outs;
+    for (Column* c : whole.t->cols) { col_incref(c); outs.v.push_back(c); }
+    for (Column* c : fns.t->cols) { col_incref(c); outs.v.push_back(c); }
+    TableRef out(new_table(outs.release()));
+    context = std::move(nc);
+    waiting_rows -= rows;
+    waiting.pop_front();
+    return out.release();
+  }
+  // bounded: an OOM halves the front batch; the halves wait in its place and leave as two output batches
+  Table* run_bounded() {
+    while (true) {
+      try {
+        return run_front();
+      } catch (const Error& e) {
+        if (!splittable(e) || waiting.front().rows < 2) throw;
+        note_split();
+        TableRef whole(waiting.front().get());
+        const int64_t n = whole.t->rows, h = n / 2;
+        TableRef a(with_retry([&] { return slice_table(whole.t, 0, h); }));
+        TableRef b(with_retry([&] { return slice_table(whole.t, h, n); }));
+        SpillPiece pa, pb;
+        pa.hold(a.t);
+        pb.hold(b.t);
+        waiting.pop_front();
+        waiting.push_front(std::move(pb));
+        waiting.push_front(std::move(pa));
+      }
+    }
+  }
+  Table* next_bounded() {
+    while (true) {
+      if (!waiting.empty() && (done || waiting_rows - waiting.front().rows >= plan.post)) return run_bounded();
+      if (done) return nullptr;
+      TableRef in(children[0]->next());
+      if (!in.t) { done = true; continue; }
+      if (in.t->rows == 0) continue;
+      if (!bound) { bind_window(plan, in.t); read_cols = window_read_columns(plan, &chunk_plan); bound = true; }
+      SpillPiece p;
+      p.hold(in.t);
+      waiting_rows += in.t->rows;
+      waiting.push_back(std::move(p));
+    }
+  }
   Table* do_next() override {
+    if (plan.bounded) return next_bounded();
     if (!pending.empty()) {
       TableRef t(std::move(pending.front()));
       pending.pop_front();

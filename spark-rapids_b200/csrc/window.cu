@@ -16,6 +16,8 @@
 //                             at the partition's end), a difference of prefixes for integer, decimal and count sums, otherwise a
 //                             loop over the frame (float SUM, MIN, MAX: O(rows x frame width), as cudf's rolling window)
 //   window_lead_lag_kernel    LEAD / LAG source row (or -1 outside the partition); values through gather_table, then the default
+// Finish and LEAD / LAG run over every row of the chunk (AllRows) or, for a streamed bounded plan, only over the rows [lo, hi)
+// between its context and look-ahead rows (RowRange), writing columns of hi - lo rows.
 #include <algorithm>
 #include "sortkey.cuh"
 #include "window.cuh"
@@ -368,11 +370,33 @@ __global__ void window_group_ends_kernel(const uint8_t* __restrict__ flags, cons
   }
 }
 
-template <class Op>
-__global__ void window_finish_kernel(const Op op, const FrameArgs fr, const Groups g, const typename Op::T* __restrict__ state, int64_t n,
+// The rows a finish or LEAD / LAG launch writes: every row of the chunk, or only [lo, hi) (the rest are context and look-ahead
+// rows of a streamed bounded plan, read but never written), into columns of hi - lo rows
+struct AllRows {
+  int64_t n;
+  __device__ __forceinline__ int64_t begin() const { return 0; }
+  __device__ __forceinline__ int64_t end() const { return n; }
+  __device__ __forceinline__ int64_t out(int64_t i) const { return i; }
+};
+struct RowRange {
+  int64_t lo, hi;
+  __device__ __forceinline__ int64_t begin() const { return lo; }
+  __device__ __forceinline__ int64_t end() const { return hi; }
+  __device__ __forceinline__ int64_t out(int64_t i) const { return i - lo; }
+};
+
+// With a carry, rank[i].rn counts from the partition's true start, so ps = i - rn + 1 is clipped to 0 for a partition that began
+// in an earlier chunk, and pend_at[0] is then the chunk's last row of it.  Over RowRange rows of a streamed bounded plan neither
+// cuts a frame short: the chunk holds P + 1 rows before lo (or every row since the input began, when ps is exact) and F rows
+// after hi - 1 (or every row up to the input's end, when pe is exact), so every output row has i + lower >= 1 and
+// i + upper <= n - 1.  So s = i + lower >= 1 > ps whenever ps was clipped: such a frame is never from_start and its difference
+// of prefixes reads state[s - 1] inside the chunk, where both prefixes include the carry alike.  A frame from UNBOUNDED
+// PRECEDING is from_start and reads state[e], which continues the carry as a running frame does.
+template <class Op, class R>
+__global__ void window_finish_kernel(const Op op, const FrameArgs fr, const Groups g, const typename Op::T* __restrict__ state, const R rows,
                                      const WinOut out) {
   using T = typename Op::T;
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+  for (int64_t i = rows.begin() + blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < rows.end(); i += (int64_t)gridDim.x * blockDim.x) {
     int64_t s = 0, e = i;
     bool from_start = true, empty = false;
     if (fr.type == FR_RANGE_RUNNING) {
@@ -393,15 +417,17 @@ __global__ void window_finish_kernel(const Op op, const FrameArgs fr, const Grou
       v = op.identity();
       for (int64_t j = s; j <= e; j++) v = op.combine(v, op.elem(j));
     }
-    op.finish(v, fr.type != FR_GENERAL, out, i);
+    op.finish(v, fr.type != FR_GENERAL, out, rows.out(i));
   }
 }
 
-__global__ void window_lead_lag_kernel(const RankOp::T* __restrict__ rank, const int32_t* __restrict__ pend_at, int64_t n, int64_t off,
+// map[out(i)] = the source row of row i in the chunk, or -1 outside the partition
+template <class R>
+__global__ void window_lead_lag_kernel(const RankOp::T* __restrict__ rank, const int32_t* __restrict__ pend_at, const R rows, int64_t off,
                                        int32_t* __restrict__ map) {
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+  for (int64_t i = rows.begin() + blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < rows.end(); i += (int64_t)gridDim.x * blockDim.x) {
     const int64_t ps = max((int64_t)0, i - rank[i].rn + 1), pe = pend_at[ps], src = i + off;
-    map[i] = (src >= ps && src <= pe) ? (int32_t)src : -1;
+    map[rows.out(i)] = (src >= ps && src <= pe) ? (int32_t)src : -1;
   }
 }
 
@@ -428,6 +454,10 @@ WindowPlan make_window_plan(const int32_t* part_cols, int nparts, const b2_order
   p.part.assign(part_cols, part_cols + nparts);
   p.order.assign(order, order + norder);
   p.mode = 1;
+  // the row extents of the streamed bounded class: offsets clamped as frame_args clamps them, so P + F cannot overflow
+  const int64_t lim = (int64_t)1 << 40;
+  auto clamp = [&](int64_t v) { return std::max(-lim, std::min(lim, v)); };
+  bool streamable = true;
   for (int k = 0; k < nspecs; k++) {
     WinFn f;
     f.s = specs[k];
@@ -453,9 +483,39 @@ WindowPlan make_window_plan(const int32_t* part_cols, int nparts, const b2_order
     }
     const int m = (f.frame == FR_GENERAL) ? 3 : f.frame == FR_RANGE_RUNNING ? 2 : 1;
     p.mode = std::max(p.mode, m);
+    if (kind == B2_WIN_LAG) p.pre = std::max(p.pre, (int64_t)f.s.offset);
+    else if (kind == B2_WIN_LEAD) p.post = std::max(p.post, (int64_t)f.s.offset);
+    else if (!is_ranking(kind)) {
+      if (f.s.frame != B2_FRAME_ROWS || f.s.upper == B2_UNBOUNDED_FOLLOWING) {
+        streamable = false;
+      } else {
+        // UNBOUNDED PRECEDING -> u reads the scan state at row i + u; [l, u] reads the rows between i + l and i + u
+        const int64_t u = clamp(f.s.upper), l = f.s.lower == B2_UNBOUNDED_PRECEDING ? u : clamp(f.s.lower);
+        p.pre = std::max(p.pre, std::max(-l, -u));
+        p.post = std::max(p.post, std::max(l, u));
+      }
+    }
     p.fns.push_back(f);
   }
+  p.bounded = streamable && p.pre + p.post > 0;
   return p;
+}
+
+// the columns the plan reads (partition keys, order keys, function inputs; each once) and the plan over a table of just those
+std::vector<int> window_read_columns(const WindowPlan& p, WindowPlan* over_read) {
+  std::vector<int> cols;
+  auto at = [&](int c) -> int32_t {
+    for (size_t k = 0; k < cols.size(); k++)
+      if (cols[k] == c) return (int32_t)k;
+    cols.push_back(c);
+    return (int32_t)cols.size() - 1;
+  };
+  *over_read = p;
+  for (int32_t& c : over_read->part) c = at(c);
+  for (auto& o : over_read->order) o.column = at(o.column);
+  for (WinFn& f : over_read->fns)
+    if (needs_column(f.s.kind)) f.s.column = at(f.s.column);
+  return cols;
 }
 
 // checks the columns of the first batch against the plan
@@ -499,9 +559,15 @@ static DevBuf run_scan(const Op& op, const uint8_t* flags, int64_t n, const DevB
   return state;
 }
 
+// the output rows of a chunk and the row the carry is taken at (rows = null: every row, carry at the last)
+struct ChunkRows { int64_t lo, hi, carry_row; };
+
 template <class Op>
-static void run_finish(const Op& op, const FrameArgs& fr, const Groups& g, const DevBuf& state, int64_t n, const WinOut& o) {
-  launch("window_finish_kernel", window_finish_kernel<Op>, grid_for(n, 256), 256, 0, stream(), op, fr, g, state.as<typename Op::T>(), n, o);
+static void run_finish(const Op& op, const FrameArgs& fr, const Groups& g, const DevBuf& state, int64_t n, const WinOut& o, const ChunkRows* rows) {
+  using T = typename Op::T;
+  if (!rows) launch("window_finish_kernel", window_finish_kernel<Op, AllRows>, grid_for(n, 256), 256, 0, stream(), op, fr, g, state.as<T>(), AllRows{n}, o);
+  else launch("window_finish_kernel", window_finish_kernel<Op, RowRange>, grid_for(rows->hi - rows->lo, 256), 256, 0, stream(), op, fr, g, state.as<T>(),
+              RowRange{rows->lo, rows->hi}, o);
 }
 
 static SortPlan empty_plan() { SortPlan p; memset(&p, 0, sizeof(p)); return p; }
@@ -548,11 +614,20 @@ static FrameArgs frame_args(const WinFn& f) {
   return fr;
 }
 
-// One chunk of rows sorted by (partition, order): the input columns, then one column per function.  With a carry, row 0 continues
-// the partition the previous chunk ended with (when its keys say so) and the carry is replaced by this chunk's on success.
-Table* window_chunk(WindowPlan& p, const Table* t, WindowCarry* carry) {
+// the state at row r of a scan (r >= 0) as the carry of that function, copied on the device
+template <typename T>
+static void carry_at(const DevBuf& state, int64_t r, DevBuf& carry) {
+  CUDA_CHECK(cudaMemcpyAsync(carry.p, state.as<char>() + (size_t)r * sizeof(T), sizeof(T), cudaMemcpyDeviceToDevice, stream()));
+}
+
+// The functions over one chunk of rows sorted by (partition, order), one column per function.  With `rows`, only the rows
+// [lo, hi) are written (columns of hi - lo rows) and the carry is taken at rows->carry_row (-1: the carry passed in stays);
+// otherwise every row, and the carry at the last row.  The carry is replaced only on success.
+static std::vector<Column*> window_functions(WindowPlan& p, const Table* t, WindowCarry* carry, const ChunkRows* rows) {
   const int64_t n = t->rows;
   if (n > 0x7fffffffLL) throw Error(B2_ERR_SIZE_OVERFLOW, "window over more than 2^31-1 rows");
+  const int64_t lo = rows ? rows->lo : 0, hi = rows ? rows->hi : n, m = hi - lo;
+  const int64_t carry_row = rows ? rows->carry_row : n - 1;
   const size_t nf = p.fns.size();
   const Table* last = carry ? carry->last : nullptr;
   const bool has_state = carry && !carry->state.empty();
@@ -562,6 +637,7 @@ Table* window_chunk(WindowPlan& p, const Table* t, WindowCarry* carry) {
 
   RankOp rop{fl};
   DevBuf rank = n ? run_scan(rop, fl, n, has_state ? &carry->state[0] : nullptr, next_state[0]) : DevBuf();
+  if (rows && carry_row >= 0) carry_at<RankOp::T>(rank, carry_row, next_state[0]);
   bool need_pend = false, need_peer = false;
   for (const WinFn& f : p.fns) { need_pend = need_pend || f.frame == FR_GENERAL; need_peer = need_peer || f.frame == FR_RANGE_RUNNING; }
   DevBuf pend, peer;
@@ -574,26 +650,29 @@ Table* window_chunk(WindowPlan& p, const Table* t, WindowCarry* carry) {
   const Groups g{rank.as<RankOp::T>(), pend.as<int32_t>(), peer.as<int32_t>()};
 
   ColsGuard outs;
-  for (Column* c : t->cols) { col_incref(c); outs.v.push_back(c); }
   for (size_t k = 0; k < nf; k++) {
     const WinFn& f = p.fns[k];
     const int kind = f.s.kind;
     const DevBuf* cin = has_state && carry->state[k + 1].p ? &carry->state[k + 1] : nullptr;
     const Column* in = needs_column(kind) ? t->cols[f.s.column] : nullptr;
     if (is_offset_fn(kind)) {
-      DevBuf map((size_t)std::max<int64_t>(n, 1) * 4);
+      DevBuf map((size_t)std::max<int64_t>(m, 1) * 4);
       const int64_t off = kind == B2_WIN_LEAD ? (int64_t)f.s.offset : -(int64_t)f.s.offset;
-      if (n) launch("window_lead_lag_kernel", window_lead_lag_kernel, grid_for(n, 256), 256, 0, stream(), rank.as<RankOp::T>(), pend.as<int32_t>(), n, off,
-                    map.as<int32_t>());
+      if (m && !rows)
+        launch("window_lead_lag_kernel", window_lead_lag_kernel<AllRows>, grid_for(n, 256), 256, 0, stream(), rank.as<RankOp::T>(), pend.as<int32_t>(),
+               AllRows{n}, off, map.as<int32_t>());
+      else if (m)
+        launch("window_lead_lag_kernel", window_lead_lag_kernel<RowRange>, grid_for(m, 256), 256, 0, stream(), rank.as<RankOp::T>(), pend.as<int32_t>(),
+               RowRange{lo, hi}, off, map.as<int32_t>());
       std::vector<int> only{f.s.column};
-      std::unique_ptr<Table, void (*)(Table*)> got(gather_table(t, map.as<int32_t>(), n, true, &only), table_release);
+      std::unique_ptr<Table, void (*)(Table*)> got(gather_table(t, map.as<int32_t>(), m, true, &only), table_release);
       Column* c = got->cols[0];
       col_incref(c);
       outs.v.push_back(c);
-      if (!f.s.default_is_null && n) {
+      if (!f.s.default_is_null && m) {
         uint4 d;
         memcpy(&d, f.s.default_value, 16);
-        launch("window_default_kernel", window_default_kernel, grid_for(n, 256), 256, 0, stream(), map.as<int32_t>(), n, dtype_width(c->dtype), d, c->data.p,
+        launch("window_default_kernel", window_default_kernel, grid_for(m, 256), 256, 0, stream(), map.as<int32_t>(), m, dtype_width(c->dtype), d, c->data.p,
                c->valid.as<uint32_t>());
       }
       finalize_nulls(c);
@@ -605,45 +684,49 @@ Table* window_chunk(WindowPlan& p, const Table* t, WindowCarry* carry) {
       if (is_decimal(f.in_dtype)) { odt = f.s.out_dtype; oscale = in->scale; }
       else if (is_float(f.in_dtype)) odt = B2_FLOAT64;
     } else if (kind == B2_WIN_MIN || kind == B2_WIN_MAX) { odt = in->dtype; oscale = in->scale; }
-    Column* oc = new_column(odt, oscale, n, true);
+    Column* oc = new_column(odt, oscale, m, true);
     outs.v.push_back(oc);
-    if (n == 0) { finalize_nulls(oc); continue; }
+    if (m == 0) { finalize_nulls(oc); continue; }
     CUDA_CHECK(cudaMemsetAsync(oc->valid.p, 0, oc->valid.bytes, stream()));
     const WinOut o{oc->data.p, oc->valid.as<uint32_t>(), odt, f.s.out_precision, kind == B2_WIN_ROW_NUMBER ? 0 : kind == B2_WIN_RANK ? 1 : 2};
     const FrameArgs fr = frame_args(f);
-    if (is_ranking(kind)) {
-      run_finish(rop, fr, g, rank, n, o);
-    } else if (kind == B2_WIN_COUNT || kind == B2_WIN_COUNT_ALL) {
-      CountOp op{in ? view_of(in) : ColView{}, kind == B2_WIN_COUNT_ALL};
+    auto scan_finish = [&](const auto& op) {
+      using T = typename std::decay_t<decltype(op)>::T;
       DevBuf st = run_scan(op, fl, n, cin, next_state[k + 1]);
-      run_finish(op, fr, g, st, n, o);
-    } else if (kind == B2_WIN_SUM && is_decimal(f.in_dtype)) {
-      SumDecOp op{view_of(in)};
-      DevBuf st = run_scan(op, fl, n, cin, next_state[k + 1]);
-      run_finish(op, fr, g, st, n, o);
-    } else if (kind == B2_WIN_SUM && is_float(f.in_dtype)) {
-      SumFloatOp op{view_of(in)};
-      DevBuf st = run_scan(op, fl, n, cin, next_state[k + 1]);
-      run_finish(op, fr, g, st, n, o);
-    } else if (kind == B2_WIN_SUM) {
-      SumIntOp op{view_of(in)};
-      DevBuf st = run_scan(op, fl, n, cin, next_state[k + 1]);
-      run_finish(op, fr, g, st, n, o);
-    } else {
-      MinMaxOp op{view_of(in), kind == B2_WIN_MAX};
-      DevBuf st = run_scan(op, fl, n, cin, next_state[k + 1]);
-      run_finish(op, fr, g, st, n, o);
-    }
+      if (rows && carry_row >= 0) carry_at<T>(st, carry_row, next_state[k + 1]);
+      run_finish(op, fr, g, st, n, o, rows);
+    };
+    if (is_ranking(kind)) run_finish(rop, fr, g, rank, n, o, rows);
+    else if (kind == B2_WIN_COUNT || kind == B2_WIN_COUNT_ALL) scan_finish(CountOp{in ? view_of(in) : ColView{}, kind == B2_WIN_COUNT_ALL});
+    else if (kind == B2_WIN_SUM && is_decimal(f.in_dtype)) scan_finish(SumDecOp{view_of(in)});
+    else if (kind == B2_WIN_SUM && is_float(f.in_dtype)) scan_finish(SumFloatOp{view_of(in)});
+    else if (kind == B2_WIN_SUM) scan_finish(SumIntOp{view_of(in)});
+    else scan_finish(MinMaxOp{view_of(in), kind == B2_WIN_MAX});
     finalize_nulls(oc);
   }
-  std::unique_ptr<Table, void (*)(Table*)> out(new_table(outs.release()), table_release);
-  if (carry && n) {   // replaced only now, so that a failed attempt leaves the carry as it was
-    Table* nl = slice_table(t, n - 1, n);
+  if (carry && n && carry_row >= 0) {   // replaced only now, so that a failed attempt leaves the carry as it was
+    Table* nl = slice_table(t, carry_row, carry_row + 1);
     if (carry->last) table_release(carry->last);
     carry->last = nl;
     carry->state = std::move(next_state);
   }
-  return out.release();
+  return outs.release();
+}
+
+// One chunk of rows sorted by (partition, order): the input columns, then one column per function.  With a carry, row 0 continues
+// the partition the previous chunk ended with (when its keys say so) and the carry is replaced by this chunk's on success.
+Table* window_chunk(WindowPlan& p, const Table* t, WindowCarry* carry) {
+  std::vector<Column*> fns = window_functions(p, t, carry, nullptr);
+  ColsGuard outs;
+  for (Column* c : t->cols) { col_incref(c); outs.v.push_back(c); }
+  outs.v.insert(outs.v.end(), fns.begin(), fns.end());
+  return new_table(outs.release());
+}
+
+Table* window_chunk_rows(WindowPlan& p, const Table* t, WindowCarry* carry, int64_t lo, int64_t hi, int64_t carry_row) {
+  B2_CHECK(lo >= 0 && lo <= hi && hi <= t->rows && carry_row >= -1 && carry_row < t->rows, "window: chunk rows out of range");
+  const ChunkRows rows{lo, hi, carry_row};
+  return new_table(window_functions(p, t, carry, &rows));
 }
 
 }  // namespace b2
