@@ -24,7 +24,9 @@ def arrow_to_ocol(col):
     valid = np.array([v is not None for v in col.to_pylist()], dtype=bool) if col.null_count else np.ones(n, bool)
     if pa.types.is_decimal(typ):
         dt = O.decimal_dtype_for(typ.precision)
-        vals = np.array([0 if v is None else int(decimal.Decimal(v).scaleb(typ.scale)) for v in col.to_pylist()], dtype=object)
+        # exact: the default decimal context keeps 28 digits and would round DECIMAL(29..38) values
+        exact = decimal.Context(prec=80)
+        vals = np.array([0 if v is None else int(decimal.Decimal(v).scaleb(typ.scale, exact)) for v in col.to_pylist()], dtype=object)
         return O.OCol(vals, valid, (dt, typ.precision, typ.scale))
     if pa.types.is_string(typ) or pa.types.is_binary(typ) or pa.types.is_large_string(typ):
         vals = np.array([b"" if v is None else (v if isinstance(v, bytes) else v.encode()) for v in col.to_pylist()], dtype=object)

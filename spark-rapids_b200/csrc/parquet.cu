@@ -639,9 +639,13 @@ __device__ __forceinline__ uint32_t extract_bits(const uint8_t* data, uint64_t b
   return (uint32_t)(v & ((bw >= 32) ? 0xffffffffull : ((1ull << bw) - 1)));
 }
 
-// CTA-cooperative decode of `count` values; Sink::put(k, v) is called once per value by some thread
+// CTA-cooperative decode of `count` values; Sink::put(k, v) is called once per value by some thread.
+// Untrusted input: a stream that ends before `count` values (or with a zero-length run), and a run whose values
+// lie past `end`, set *errors = 6 — rows it does not cover are left unwritten, so the decode fails before anything
+// reads those rows (parquet_decode's check_err).  A bit-packed run may announce more groups than the stream holds
+// as long as the values it supplies are inside.
 template <typename Sink>
-__device__ void decode_hybrid(const uint8_t* p, const uint8_t* end, int bw, int count, Sink& sink) {
+__device__ void decode_hybrid(const uint8_t* p, const uint8_t* end, int bw, int count, Sink& sink, int32_t* errors) {
   __shared__ RunD s_runs[PQ_RUNS];
   __shared__ int s_nruns, s_done;
   __shared__ const uint8_t* s_pos;
@@ -652,17 +656,26 @@ __device__ void decode_hybrid(const uint8_t* p, const uint8_t* end, int bw, int 
     if (threadIdx.x == 0) {
       const uint8_t* q = s_pos;
       int done = s_done, n = 0;
+      bool bad = false;
       while (n < PQ_RUNS && done < count && q < end) {
         uint32_t h = 0; int shift = 0;
-        while (q < end) { uint8_t b = *q++; h |= (uint32_t)(b & 0x7f) << shift; if (!(b & 0x80)) break; shift += 7; }
+        while (q < end && shift < 32) { uint8_t b = *q++; h |= (uint32_t)(b & 0x7f) << shift; if (!(b & 0x80)) break; shift += 7; }
         RunD r; r.start = done;
-        if (h & 1) { const int groups = (int)(h >> 1); r.packed = 1; r.count = min(groups * 8, count - done); r.data = q; r.value = 0; q += (size_t)groups * bw; }
-        else { r.packed = 0; r.count = min((int)(h >> 1), count - done); uint32_t v = 0; for (int k = 0; k < vbytes && q < end; k++) v |= (uint32_t)(*q++) << (8 * k); r.value = v; r.data = nullptr; }
-        if (r.count <= 0) { if (!(h & 1) && (h >> 1) == 0) { done = count; } break; }
+        if (h & 1) {
+          const int64_t groups = h >> 1;
+          r.packed = 1; r.count = (int)min(groups * 8, (int64_t)(count - done)); r.data = q; r.value = 0;
+          if (((int64_t)r.count * bw + 7) / 8 > end - q) { bad = true; break; }
+          q += min(groups * bw, (int64_t)(end - q));
+        } else {
+          r.packed = 0; r.count = (int)min((int64_t)(h >> 1), (int64_t)(count - done));
+          if (vbytes > end - q) { bad = true; break; }
+          uint32_t v = 0; for (int k = 0; k < vbytes; k++) v |= (uint32_t)(*q++) << (8 * k); r.value = v; r.data = nullptr;
+        }
+        if (r.count <= 0) { q = end; break; }   // a zero-length run ends the stream
         done += r.count;
         s_runs[n++] = r;
       }
-      if (n == 0) done = count;  // malformed / exhausted stream: stop
+      if (bad || (n == 0 && done < count)) { atomicExch(errors, 6); done = count; }
       s_nruns = n; s_done = done; s_pos = q;
     }
     __syncthreads();
@@ -692,15 +705,20 @@ struct LevelSink {
   __device__ __forceinline__ void put(int k, uint32_t v) { const bool ok = (int)v == max_def; lvl[k] = ok; if (ok) atomicAdd(cnt, 1u); }
   __device__ __forceinline__ void put4(int k, uint32_t a, uint32_t b, uint32_t c, uint32_t d) { put(k, a); put(k + 32, b); put(k + 64, c); put(k + 96, d); }
 };
-__device__ __forceinline__ const uint8_t* levels_of(const PageD& pg, const uint8_t* d, const uint8_t*& lv_end, const uint8_t*& values) {
-  if (pg.kind == PG_DATA_V2) { lv_end = d + pg.lvl_bytes; values = d + pg.lvl_bytes; return d; }
-  uint32_t n; memcpy(&n, d, 4);
-  lv_end = d + 4 + n; values = d + 4 + n;
-  return d + 4;
+// definition levels [lv, lv_end) and the values behind them.  V1 pages prefix the levels with their 4-byte length;
+// false when that prefix (or its length) runs past the page
+__device__ __forceinline__ bool levels_of(const PageD& pg, const uint8_t* d, const uint8_t*& lv, const uint8_t*& lv_end, const uint8_t*& values) {
+  if (pg.kind == PG_DATA_V2) { lv = d; lv_end = d + pg.lvl_bytes; values = d + pg.lvl_bytes; return true; }
+  uint32_t n = 0;
+  if (pg.uncomp_size >= 4) memcpy(&n, d, 4);
+  const bool ok = pg.uncomp_size >= 4 && n <= (uint32_t)pg.uncomp_size - 4;
+  if (!ok) n = 0;
+  lv = d + 4; lv_end = d + 4 + n; values = d + 4 + n;
+  return ok;
 }
 __global__ void __launch_bounds__(PQ_NT) levels_kernel(const PageD* __restrict__ pages, const int32_t* __restrict__ todo, const ChunkD* __restrict__ chunks,
                                                        const ColD* __restrict__ cols, const uint8_t* __restrict__ file, const uint8_t* __restrict__ scratch,
-                                                       int32_t* __restrict__ nonnull) {
+                                                       int32_t* __restrict__ nonnull, int32_t* __restrict__ errors) {
   __shared__ unsigned int s_cnt;
   const int pi = todo[blockIdx.x];
   const PageD pg = pages[pi];
@@ -708,8 +726,8 @@ __global__ void __launch_bounds__(PQ_NT) levels_kernel(const PageD* __restrict__
   if (threadIdx.x == 0) s_cnt = 0;
   __syncthreads();
   const uint8_t* d = page_ptr(pg, file, scratch);
-  const uint8_t *lv_end, *vals;
-  const uint8_t* lv = levels_of(pg, d, lv_end, vals);
+  const uint8_t *lv, *lv_end, *vals;
+  if (!levels_of(pg, d, lv, lv_end, vals)) { if (threadIdx.x == 0) { nonnull[pi] = 0; atomicExch(errors, 7); } return; }
   uint8_t* out_lvl = cols[ch.col].lvl + pg.row_start;
   // the usual page of a nullable column without NULLs: one RLE run "every level = max_def" — no per-row work
   {
@@ -725,7 +743,7 @@ __global__ void __launch_bounds__(PQ_NT) levels_kernel(const PageD* __restrict__
     }
   }
   LevelSink sink{out_lvl, ch.max_def, &s_cnt};
-  decode_hybrid(lv, lv_end, 1, pg.num_values, sink);  // flat schema: max_def == 1 -> bit width 1
+  decode_hybrid(lv, lv_end, 1, pg.num_values, sink, errors);  // flat schema: max_def == 1 -> bit width 1
   __syncthreads();
   if (threadIdx.x == 0) nonnull[pi] = (int32_t)s_cnt;
 }
@@ -928,9 +946,12 @@ __global__ void __launch_bounds__(PQ_NT) values_kernel(const PageD* __restrict__
   const uint8_t* d = page_ptr(pg, file, scratch);
   const uint8_t* vals = d;
   const uint8_t* pend = d + pg.uncomp_size;
-  if (ch.max_def > 0) { const uint8_t* lv_end; levels_of(pg, d, lv_end, vals); }
-  else if (pg.kind == PG_DATA_V2) vals = d + pg.lvl_bytes;
+  if (ch.max_def > 0) {
+    const uint8_t *lv, *lv_end;
+    if (!levels_of(pg, d, lv, lv_end, vals)) return;   // levels_kernel reported the page
+  } else if (pg.kind == PG_DATA_V2) vals = d + pg.lvl_bytes;
   const int nvals = ch.max_def > 0 ? nonnull[pi] : pg.num_values;
+  if (nvals == 0) return;   // an all-NULL page: its value stream may be empty (no dictionary bit width, no length prefix)
   ValueWriter w; w.col = col; w.base = pg.value_base; w.dict = nullptr; w.dict_count = 0;
   w.dict_src = dict_src + ch.dict_str_off; w.dict_len = dict_len + ch.dict_str_off;
   const int src_width = ch.phys == PT_INT32 || ch.phys == PT_FLOAT ? 4 : (ch.phys == PT_FLBA ? ch.type_length : 8);
@@ -938,12 +959,14 @@ __global__ void __launch_bounds__(PQ_NT) values_kernel(const PageD* __restrict__
     if (ch.dict_page < 0) { if (threadIdx.x == 0) atomicExch(errors, 3); return; }
     w.dict = page_ptr(pages[ch.dict_page], file, scratch);
     w.dict_count = ch.dict_count;
+    if (vals >= pend || vals[0] > 32) { if (threadIdx.x == 0) atomicExch(errors, 6); return; }
     const int bw = vals[0];
     DictSink sink{w, src_width, errors};
     if (bw == 0) { for (int k = threadIdx.x; k < nvals; k += PQ_NT) sink.put(k, 0); }
-    else decode_hybrid(vals + 1, pend, bw, nvals, sink);
+    else decode_hybrid(vals + 1, pend, bw, nvals, sink, errors);
   } else if (pg.encoding == ENC_PLAIN) {
     if (ch.phys == PT_BOOLEAN) {
+      if (vals > pend || (size_t)(nvals + 7) / 8 > (size_t)(pend - vals)) { if (threadIdx.x == 0) atomicExch(errors, 5); return; }
       for (int k = threadIdx.x; k < nvals; k += PQ_NT) reinterpret_cast<int8_t*>(col.dense)[w.base + k] = (vals[k >> 3] >> (k & 7)) & 1;
     } else if (ch.phys == PT_BYTE_ARRAY) {
       // length-prefixed values: a sequential walk (dictionary pages normally carry the strings)
@@ -977,7 +1000,10 @@ __global__ void __launch_bounds__(PQ_NT) values_kernel(const PageD* __restrict__
       __device__ __forceinline__ void put4(int k, uint32_t a, uint32_t b, uint32_t c, uint32_t d) { put(k, a); put(k + 32, b); put(k + 64, c); put(k + 96, d); }
     };
     BoolSink sink{reinterpret_cast<int8_t*>(col.dense) + w.base};
-    decode_hybrid(vals + 4, pend, 1, nvals, sink);
+    uint32_t n = 0;
+    if (vals <= pend && pend - vals >= 4) memcpy(&n, vals, 4);
+    if (vals > pend || pend - vals < 4 || n > (uint32_t)(pend - vals - 4)) { if (threadIdx.x == 0) atomicExch(errors, 6); return; }
+    decode_hybrid(vals + 4, vals + 4 + n, 1, nvals, sink, errors);
   } else {
     if (threadIdx.x == 0) atomicExch(errors, 4);
   }
@@ -1069,7 +1095,8 @@ static OutColPlan plan_column(const SchemaElem& e, int schema_idx) {
       break;
     case PT_INT64:
       p.out_width = 8; p.conv = 0;
-      if (dec) { p.out_dtype = B2_DECIMAL64; p.out_scale = e.scale; }
+      if (dec && e.precision <= 9) { p.out_dtype = B2_DECIMAL32; p.out_width = 4; p.out_scale = e.scale; }   // the low 4 bytes (copy, width 4)
+      else if (dec) { p.out_dtype = B2_DECIMAL64; p.out_scale = e.scale; }
       else if (e.converted == 10 || (e.lt_timestamp && e.lt_ts_unit == 2)) p.out_dtype = B2_TIMESTAMP_US;
       else if (e.converted == 9 || (e.lt_timestamp && e.lt_ts_unit == 1)) { p.out_dtype = B2_TIMESTAMP_US; p.conv = 1; }
       else if (e.lt_timestamp) throw Error(B2_ERR_UNSUPPORTED, "parquet: nanosecond timestamps");
@@ -1201,6 +1228,8 @@ Table* parquet_decode(const uint8_t* host, const uint8_t* dev_in, int64_t len, c
       pg.lvl_bytes = ptype == PG_DATA_V2 ? v2_def_len + v2_rep_len : 0;
       pg.compressed = cm.codec == CODEC_SNAPPY && (ptype != PG_DATA_V2 || v2_compressed);
       if (ptype == PG_DATA_V2 && v2_rep_len) throw Error(B2_ERR_UNSUPPORTED, "parquet: repetition levels");
+      // an uncompressed page is read in place: the decoders stop at uncompressed_page_size, which must be the bytes it has
+      if (!pg.compressed && usize != csize) throw Error(B2_ERR_INVALID, "parquet: uncompressed page sizes disagree");
       if (pg.compressed && pg.lvl_bytes == 0 && csize > usize && usize > 0) {
         // Incompressible pages (bit-packed dictionary indexes, mostly) are stored by snappy as ONE literal: the
         // page bytes sit verbatim in the file behind the length preamble and the literal header.  Read them in
@@ -1390,14 +1419,25 @@ Table* parquet_decode(const uint8_t* host, const uint8_t* dev_in, int64_t len, c
     CUDA_CHECK(cudaStreamWaitEvent(s, ev_join, 0));
     cudaEventDestroy(ev_fork); cudaEventDestroy(ev_join);
   }
+  // A corrupt page leaves rows of lvl / dense / str_src unwritten (the kernels flag it in d_err and stop).  Those
+  // bytes must never reach a kernel that indexes or dereferences through them: the flag is read at the two syncs
+  // before such kernels (after the levels pass: the scan of lvl and the NULL expansion; before string_chars_kernel:
+  // str_src holds source addresses) and at the end.
+  auto check_err = [](int32_t err) {
+    if (err == 1) throw Error(B2_ERR_INVALID, "parquet: corrupt snappy stream");
+    if (err) throw Error(B2_ERR_INVALID, "parquet: corrupt page data (code " + std::to_string(err) + ")");
+  };
   std::vector<int64_t> col_nonnull(ncols, 0);
   std::vector<bool> has_nulls(ncols, false);
   if (!todo_levels.empty()) {
     launch("levels_kernel", levels_kernel, (int)todo_levels.size(), PQ_NT, 0, s, d_pages.as<PageD>(), d_todo_l.as<int32_t>(), d_chunks.as<ChunkD>(),
-           d_cols.as<ColD>(), d_file, scratch.as<uint8_t>(), d_nonnull.as<int32_t>());
+           d_cols.as<ColD>(), d_file, scratch.as<uint8_t>(), d_nonnull.as<int32_t>(), d_err.as<int32_t>());
     std::vector<int32_t> nn(pages.size());
+    int32_t lvl_err = 0;
     d2h(nn.data(), d_nonnull.p, nn.size());
+    d2h(&lvl_err, d_err.p, 1);
     sync();
+    check_err(lvl_err);
     std::vector<int64_t> run(ncols, 0);
     for (size_t i = 0; i < pages.size(); i++) {
       PageD& pg = pages[i];
@@ -1413,13 +1453,13 @@ Table* parquet_decode(const uint8_t* host, const uint8_t* dev_in, int64_t len, c
       for (int c = 0; c < ncols; c++) hn[c] = has_nulls[c] ? 1 : 0;
       DevBuf d_hn((size_t)ncols);
       h2d(d_hn.p, hn.data(), hn.size());
-      launch(fill_uniform_levels_kernel, (int)todo_levels.size(), PQ_NT, 0, s, d_pages.as<PageD>(), d_todo_l.as<int32_t>(), d_chunks.as<ChunkD>(),
+      launch("fill_uniform_levels_kernel", fill_uniform_levels_kernel, (int)todo_levels.size(), PQ_NT, 0, s, d_pages.as<PageD>(), d_todo_l.as<int32_t>(), d_chunks.as<ChunkD>(),
              d_cols.as<ColD>(), d_nonnull.as<int32_t>(), d_hn.as<uint8_t>());
     }
   }
   DevBuf d_dict_src((size_t)std::max<int64_t>(dict_str_total, 1) * 8), d_dict_len((size_t)std::max<int64_t>(dict_str_total, 1) * 4);
   if (dict_str_total)
-    launch(dict_strings_kernel, ((int)chunks.size() + 63) / 64, 64, 0, s, d_pages.as<PageD>(), d_chunks.as<ChunkD>(), (int)chunks.size(), d_file,
+    launch("dict_strings_kernel", dict_strings_kernel, ((int)chunks.size() + 63) / 64, 64, 0, s, d_pages.as<PageD>(), d_chunks.as<ChunkD>(), (int)chunks.size(), d_file,
            scratch.as<uint8_t>(), d_dict_src.as<int64_t>(), d_dict_len.as<int32_t>(), d_err.as<int32_t>());
   if (!todo_values.empty())
     launch("values_kernel", values_kernel, (int)todo_values.size(), PQ_NT, 0, s, d_pages.as<PageD>(), d_todo_v.as<int32_t>(), d_chunks.as<ChunkD>(),
@@ -1443,25 +1483,28 @@ Table* parquet_decode(const uint8_t* host, const uint8_t* dev_in, int64_t len, c
       if (has_nulls[c]) {
         xl = DevBuf((size_t)(total_rows + 1) * 4); xs = DevBuf((size_t)std::max<int64_t>(total_rows, 1) * 8);
         if (total_rows)
-          launch(expand_null_lengths_kernel, grid_for(total_rows, 256), 256, 0, s, lvl[c].as<uint8_t>(), idx.as<int64_t>(), total_rows, lens, srcs,
+          launch("expand_null_lengths_kernel", expand_null_lengths_kernel, grid_for(total_rows, 256), 256, 0, s, lvl[c].as<uint8_t>(), idx.as<int64_t>(), total_rows, lens, srcs,
                  xl.as<int32_t>(), xs.as<int64_t>(), oc->valid.as<uint32_t>());
         lens = xl.as<int32_t>(); srcs = xs.as<int64_t>();
       }
       oc->offsets = DevBuf((size_t)(total_rows + 1) * 4);
       DevBuf sums = exclusive_scan<int32_t, int32_t>(lens, oc->offsets.as<int32_t>(), total_rows, true);
       int64_t chars = 0;
+      int32_t val_err = 0;
       d2h(&chars, sums.as<int64_t>() + std::max<int64_t>(1, (total_rows + SCAN_TILE - 1) / SCAN_TILE), 1);
+      d2h(&val_err, d_err.p, 1);
       sync();
+      check_err(val_err);
       if (chars > 0x7fffffffLL) throw Error(B2_ERR_SIZE_OVERFLOW, "parquet: string column exceeds 2^31-1 chars");
       oc->chars_bytes = chars;
       oc->data = DevBuf((size_t)chars);
       if (chars) {
-        launch(string_chars_kernel, grid_for(total_rows * 32, 256), 256, 0, s, srcs, oc->offsets.as<int32_t>(), total_rows, oc->data.as<uint8_t>());
+        launch("string_chars_kernel", string_chars_kernel, grid_for(total_rows * 32, 256), 256, 0, s, srcs, oc->offsets.as<int32_t>(), total_rows, oc->data.as<uint8_t>());
         sync();  // srcs / scratch are read by the kernel; keep them alive
       }
     } else if (has_nulls[c]) {
       oc->data = DevBuf((size_t)total_rows * plans[c].out_width);
-      launch(expand_nulls_kernel, grid_for(total_rows, 256), 256, 0, s, lvl[c].as<uint8_t>(), idx.as<int64_t>(), total_rows, plans[c].out_width,
+      launch("expand_nulls_kernel", expand_nulls_kernel, grid_for(total_rows, 256), 256, 0, s, lvl[c].as<uint8_t>(), idx.as<int64_t>(), total_rows, plans[c].out_width,
              dense[c].as<uint8_t>(), oc->data.as<uint8_t>(), oc->valid.as<uint32_t>());
     } else {
       oc->data = std::move(dense[c]);  // no NULLs: the dense decode IS the column
@@ -1472,8 +1515,7 @@ Table* parquet_decode(const uint8_t* host, const uint8_t* dev_in, int64_t len, c
   int32_t err = 0;
   d2h(&err, d_err.p, 1);
   sync();
-  if (err == 1) throw Error(B2_ERR_INVALID, "parquet: corrupt snappy stream");
-  if (err) throw Error(B2_ERR_INVALID, "parquet: corrupt page data (code " + std::to_string(err) + ")");
+  check_err(err);
   return new_table(outs.release());
 }
 
