@@ -692,7 +692,7 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
       em_packed = true;
       std::vector<int> bcols = build_out;
       if (!pruned) for (int c = 0; c < (int)build_table.t->cols.size(); c++) bcols.push_back(c);
-      try { em_ok = join_pack_payload(build_table.t, bcols, em_payload); }
+      try { em_ok = join_pack_payload(ht, build_table.t, bcols, em_payload); }
       catch (const Error& e) { if (e.code != B2_ERR_OOM) throw; em_ok = false; em_payload = JoinPayload(); }   // no room: the maps
     }
     if (!em_ok) return nullptr;

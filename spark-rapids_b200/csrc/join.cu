@@ -7,7 +7,10 @@
 // The reference API takes both key tables on every call, so the hash table is rebuilt for every
 // stream batch.  Here the build side is hashed ONCE into a persistent open-addressing multimap
 // (8-byte slots: 32-bit hash tag + 32-bit build row) that any number of probe calls reuse.
-// Probe is count -> scan -> write so the gather maps are exactly sized and ordered by stream row.
+// Probe is count -> scan -> write so the gather maps are exactly sized and ordered by stream row.  A build side of one dense,
+// distinct integer key column gets a direct table instead: an exact bitmap with block ranks (DIRECT_MAX_BITS, direct_build).
+#include <atomic>
+#include <mutex>
 #include <type_traits>
 #include "joinemit.cuh"
 #include "prim.cuh"
@@ -36,8 +39,68 @@ struct JoinTable {
   DevBuf bloom;
   uint32_t bloom_mask = 0;  // 64-bit words - 1; 0 = no filter
   std::vector<int> key_idx;
+  // slots (and Bloom filter) built: at b2_join_build, except on a direct table, which builds them on the first probe that has no
+  // direct variant (ensure_hash).  A table is shared by task threads, each on its own stream: that lazy build is the one write
+  // after b2_join_build, done once under hash_mu and published by `hashed` once its stream has finished it
+  std::atomic<bool> hashed{false};
+  std::mutex hash_mu;
+  // Direct layout (b2_join_build): one distinct integer key column whose values lie in [dlo, dlo + drange) with drange at most
+  // DIRECT_DENSITY x the rows.  Key k is present iff bit k - dlo of `dbits` is set, and its rank (present keys below it) is
+  // dranks[block] + the popcount of the bits below it in its 256-bit block: a dense build index with no hash and no slot walk.
+  bool direct = false;
+  int64_t dlo = 0;
+  uint64_t drange = 0;
+  int64_t npresent = 0;     // non-NULL build keys = ranks
+  DevBuf dbits;             // uint64 words, 4 per block
+  DevBuf dranks;            // uint32 per block (+ the total)
+  DevBuf drows;             // int32 [npresent]: the build row of the key of rank i (ascending keys)
   ~JoinTable() { if (keys) table_release(keys); }
 };
+
+// what the direct probes read of a direct table
+struct DirectMap {
+  const unsigned long long* bits;
+  const uint32_t* ranks;
+  const int32_t* rows;
+  int64_t lo;
+  uint64_t range;
+};
+// the hash fields the one-key probes pass: none for a direct table, whose probes do not read them and whose lazy hash build
+// (ensure_hash) may be writing them from another thread
+struct HashView {
+  const uint64_t* slots = nullptr;
+  uint32_t mask = 0;
+  const unsigned long long* bloom = nullptr;
+  uint32_t bloom_mask = 0;
+};
+static HashView hash_view(const JoinTable* jt) {
+  HashView v;
+  if (!jt->direct) { v.slots = jt->slots.as<uint64_t>(); v.mask = (uint32_t)(jt->cap - 1); v.bloom = jt->bloom.as<unsigned long long>(); v.bloom_mask = jt->bloom_mask; }
+  return v;
+}
+static DirectMap direct_map(const JoinTable* jt) {
+  DirectMap dm; memset(&dm, 0, sizeof(dm));
+  if (jt->direct) { dm.bits = jt->dbits.as<unsigned long long>(); dm.ranks = jt->dranks.as<uint32_t>(); dm.rows = jt->drows.as<int32_t>(); dm.lo = jt->dlo; dm.range = jt->drange; }
+  return dm;
+}
+// offset of key k in the bitmap; 0xffffffff (never an offset: range <= 2^28) when k lies outside it.  The subtraction is
+// unsigned, so a key below lo wraps past the range and INT64 extremes cannot overflow
+template <typename K>
+__device__ __forceinline__ uint32_t direct_off(const DirectMap& dm, K k) {
+  const uint64_t o = (uint64_t)(int64_t)k - (uint64_t)dm.lo;
+  return o < dm.range ? (uint32_t)o : 0xffffffffu;
+}
+// rank of the present key at offset o: the block's rank + the bits below o in its (one 32-byte sector) block
+__device__ __forceinline__ uint32_t direct_rank(const DirectMap& dm, uint32_t o) {
+  const uint32_t blk = o >> 8, w = (o >> 6) & 3;
+  const ulonglong2* b = reinterpret_cast<const ulonglong2*>(dm.bits) + 2 * (size_t)blk;
+  const ulonglong2 a = __ldg(b), c = __ldg(b + 1);
+  const unsigned long long x[4] = {a.x, a.y, c.x, c.y}, below = (1ull << (o & 63)) - 1ull;
+  uint32_t rank = __ldg(&dm.ranks[blk]);
+#pragma unroll
+  for (int i = 0; i < 4; i++) rank += (uint32_t)__popcll(i < (int)w ? x[i] : (i == (int)w ? x[i] & below : 0ull));
+  return rank;
+}
 
 __device__ __forceinline__ bool any_null_key(const KeyCols& k, int64_t r) {
   for (int i = 0; i < k.n; i++) if (!row_valid(k.c[i].valid, r)) return true;
@@ -293,17 +356,29 @@ __device__ __forceinline__ void emit_row(const EmitCols& em, uint32_t o, int32_t
   }
 }
 
-template <typename K, bool TRACK, bool EMIT = false>
+// DIRECT: a direct table (DirectMap) in place of the slots and the Bloom filter.  The same phases: all key loads, then all
+// bitmap words (exact: a set bit is a match, so every queued row hits), then for the queued rows the rank from the block's
+// sector and rank word.  EMIT reads the payload at the rank (packed in rank order); the maps and TRACK use rows[rank].
+template <typename K, bool TRACK, bool EMIT = false, bool DIRECT = false>
 __device__ __forceinline__ void probe_distinct1_rows(const K* __restrict__ keys, const int32_t (&r)[PQ], const uint64_t* __restrict__ slots,
                                                      uint32_t mask, const unsigned long long* __restrict__ bloom, uint32_t bloom_mask,
                                                      unsigned long long* __restrict__ total, int32_t* __restrict__ left_map,
                                                      int32_t* __restrict__ right_map, int32_t* s_q, uint32_t* __restrict__ track,
-                                                     const EmitCols* em = nullptr) {
+                                                     const EmitCols* em = nullptr, const DirectMap* dm = nullptr) {
   typedef typename std::make_unsigned<K>::type UK;
   const int lane = threadIdx.x & 31;
   const uint32_t lt = (1u << lane) - 1u;
   uint32_t pass = 0;
-  if (bloom) {
+  if constexpr (DIRECT) {
+    uint32_t off[PQ];
+    unsigned long long wv[PQ];
+#pragma unroll
+    for (int j = 0; j < PQ; j++) off[j] = r[j] >= 0 ? direct_off(*dm, keys[r[j]]) : 0xffffffffu;
+#pragma unroll
+    for (int j = 0; j < PQ; j++) wv[j] = off[j] != 0xffffffffu ? __ldg(&dm->bits[off[j] >> 6]) : 0ull;
+#pragma unroll
+    for (int j = 0; j < PQ; j++) pass |= (uint32_t)((wv[j] >> (off[j] & 63)) & 1ull) << j;
+  } else if (bloom) {
     uint32_t h[PQ];
     unsigned long long wv[PQ];
 #pragma unroll
@@ -337,7 +412,15 @@ __device__ __forceinline__ void probe_distinct1_rows(const K* __restrict__ keys,
     const int q = q0 + lane;
     int32_t br = INT32_MIN, src = 0;
     uint64_t key = 0;   // EMIT: the key column's value
-    if (q < qn) {
+    if constexpr (DIRECT) {
+      if (q < qn) {
+        src = s_q[q];
+        const K k = keys[src];
+        key = (uint64_t)(UK)k;
+        const int32_t rank = (int32_t)direct_rank(*dm, (uint32_t)((uint64_t)(int64_t)k - (uint64_t)dm->lo));
+        br = EMIT ? rank : __ldg(&dm->rows[rank]);
+      }
+    } else if (q < qn) {
       src = s_q[q];
       const uint64_t kb = (uint64_t)(UK)keys[src];
       const uint32_t hh = hash_packed(kb);
@@ -368,12 +451,13 @@ __device__ __forceinline__ void probe_distinct1_rows(const K* __restrict__ keys,
 }
 
 // every row of the batch (SEL = false) or the rows of a selection vector (a filter below the join emitted row ids)
-template <typename K, bool SEL, bool TRACK>
+template <typename K, bool SEL, bool TRACK, bool DIRECT = false>
 __global__ void __launch_bounds__(256) join_probe_distinct1_kernel(const K* __restrict__ keys, const int32_t* __restrict__ sel, int64_t n,
                                                                    const uint64_t* __restrict__ slots, uint32_t mask,
                                                                    const unsigned long long* __restrict__ bloom, uint32_t bloom_mask,
                                                                    unsigned long long* __restrict__ total, int32_t* __restrict__ left_map,
-                                                                   int32_t* __restrict__ right_map, uint32_t* __restrict__ track) {
+                                                                   int32_t* __restrict__ right_map, uint32_t* __restrict__ track,
+                                                                   const __grid_constant__ DirectMap dm) {
   __shared__ int32_t s_q[8][32 * PQ];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
@@ -384,7 +468,7 @@ __global__ void __launch_bounds__(256) join_probe_distinct1_kernel(const K* __re
       const int64_t rr = base + j * 32 + lane;
       r[j] = rr < n ? (SEL ? sel[rr] : (int32_t)rr) : -1;
     }
-    probe_distinct1_rows<K, TRACK>(keys, r, slots, mask, bloom, bloom_mask, total, left_map, right_map, s_q[w], track);
+    probe_distinct1_rows<K, TRACK, false, DIRECT>(keys, r, slots, mask, bloom, bloom_mask, total, left_map, right_map, s_q[w], track, nullptr, &dm);
   }
 }
 
@@ -403,14 +487,15 @@ __global__ void __launch_bounds__(256) join_probe_distinct1_kernel(const K* __re
 constexpr int FP_TILE = 8 * 1024, FP_WORDS = FP_TILE / 32, FP_CTAS = 4;
 static_assert(FP_WORDS == SF_NT, "one mask word per thread");
 // EMIT: the output rows are written (EmitCols `em`) instead of the maps, which are then null
-template <typename K, bool TRACK, bool EMIT = false>
+template <typename K, bool TRACK, bool EMIT = false, bool DIRECT = false>
 __global__ void __launch_bounds__(SF_NT, FP_CTAS) join_filter_probe_kernel(const __grid_constant__ SimplePred sp, const K* __restrict__ keys, int64_t n,
                                                                           const uint64_t* __restrict__ slots, uint32_t mask,
                                                                           const unsigned long long* __restrict__ bloom, uint32_t bloom_mask,
                                                                           unsigned long long* __restrict__ total, int32_t* __restrict__ left_map,
                                                                           int32_t* __restrict__ right_map, unsigned long long* __restrict__ npass,
                                                                           uint32_t* __restrict__ track,
-                                                                          const __grid_constant__ typename std::conditional<EMIT, EmitCols, NoEmit>::type em) {
+                                                                          const __grid_constant__ typename std::conditional<EMIT, EmitCols, NoEmit>::type em,
+                                                                          const __grid_constant__ DirectMap dm) {
   __shared__ uint32_t s_mask[FP_WORDS];
   __shared__ uint16_t s_rows[FP_TILE];               // offsets in the tile of the passing rows, ascending
   __shared__ int32_t s_q[SF_NT / 32][32 * PQ];
@@ -442,8 +527,8 @@ __global__ void __launch_bounds__(SF_NT, FP_CTAS) join_filter_probe_kernel(const
         const int q = q0 + j * 32 + lane;
         r[j] = q < qn ? (int32_t)(row0 + s_rows[q]) : -1;
       }
-      if constexpr (EMIT) probe_distinct1_rows<K, TRACK, true>(keys, r, slots, mask, bloom, bloom_mask, total, left_map, right_map, s_q[w], track, &em);
-      else probe_distinct1_rows<K, TRACK>(keys, r, slots, mask, bloom, bloom_mask, total, left_map, right_map, s_q[w], track);
+      if constexpr (EMIT) probe_distinct1_rows<K, TRACK, true, DIRECT>(keys, r, slots, mask, bloom, bloom_mask, total, left_map, right_map, s_q[w], track, &em, &dm);
+      else probe_distinct1_rows<K, TRACK, false, DIRECT>(keys, r, slots, mask, bloom, bloom_mask, total, left_map, right_map, s_q[w], track, nullptr, &dm);
     }
     __syncthreads();   // s_mask, s_rows and s_wtot are rewritten by the next tile
   }
@@ -700,22 +785,25 @@ bool join_probe_pred(b2_handle ht, const Table* batch, int key_col, const Progra
   CUDA_CHECK(cudaMemsetAsync(tot.p, 0, 16, stream()));
   {
     const int grid = grid_for(n, FP_TILE, FP_CTAS);
-    const uint64_t* sl = jt->slots.as<uint64_t>(); const uint32_t msk = (uint32_t)(jt->cap - 1);
-    const unsigned long long* bl = jt->bloom.as<unsigned long long>();
+    const HashView hv = hash_view(jt);
+    const uint64_t* sl = hv.slots; const uint32_t msk = hv.mask;
+    const unsigned long long* bl = hv.bloom;
     unsigned long long* tp = tot.as<unsigned long long>();
     int32_t* lp = lm.c->data.as<int32_t>(); int32_t* rp = rm.c->data.as<int32_t>();
     const NoEmit ne;
+    const DirectMap dm = direct_map(jt);
+    const bool d = jt->direct;
     if (track) {
-      if (pw == 8) launch("join_filter_probe_track_kernel", join_filter_probe_kernel<int64_t, true>, grid, SF_NT, 0, stream(), sp, pc->data.as<int64_t>(), n,
-                          sl, msk, bl, jt->bloom_mask, tp, lp, rp, tp + 1, track, ne);
-      else launch("join_filter_probe_track_kernel", join_filter_probe_kernel<int32_t, true>, grid, SF_NT, 0, stream(), sp, pc->data.as<int32_t>(), n, sl,
-                  msk, bl, jt->bloom_mask, tp, lp, rp, tp + 1, track, ne);
+      if (pw == 8) launch("join_filter_probe_track_kernel", d ? join_filter_probe_kernel<int64_t, true, false, true> : join_filter_probe_kernel<int64_t, true>,
+                          grid, SF_NT, 0, stream(), sp, pc->data.as<int64_t>(), n, sl, msk, bl, hv.bloom_mask, tp, lp, rp, tp + 1, track, ne, dm);
+      else launch("join_filter_probe_track_kernel", d ? join_filter_probe_kernel<int32_t, true, false, true> : join_filter_probe_kernel<int32_t, true>,
+                  grid, SF_NT, 0, stream(), sp, pc->data.as<int32_t>(), n, sl, msk, bl, hv.bloom_mask, tp, lp, rp, tp + 1, track, ne, dm);
     } else if (pw == 8) {
-      launch("join_filter_probe_kernel", join_filter_probe_kernel<int64_t, false>, grid, SF_NT, 0, stream(), sp, pc->data.as<int64_t>(), n, sl, msk, bl,
-             jt->bloom_mask, tp, lp, rp, tp + 1, nullptr, ne);
+      launch("join_filter_probe_kernel", d ? join_filter_probe_kernel<int64_t, false, false, true> : join_filter_probe_kernel<int64_t, false>, grid, SF_NT, 0,
+             stream(), sp, pc->data.as<int64_t>(), n, sl, msk, bl, hv.bloom_mask, tp, lp, rp, tp + 1, nullptr, ne, dm);
     } else {
-      launch("join_filter_probe_kernel", join_filter_probe_kernel<int32_t, false>, grid, SF_NT, 0, stream(), sp, pc->data.as<int32_t>(), n, sl, msk, bl,
-             jt->bloom_mask, tp, lp, rp, tp + 1, nullptr, ne);
+      launch("join_filter_probe_kernel", d ? join_filter_probe_kernel<int32_t, false, false, true> : join_filter_probe_kernel<int32_t, false>, grid, SF_NT, 0,
+             stream(), sp, pc->data.as<int32_t>(), n, sl, msk, bl, hv.bloom_mask, tp, lp, rp, tp + 1, nullptr, ne, dm);
     }
   }
   unsigned long long h[2] = {0, 0};
@@ -734,8 +822,11 @@ struct PackCols {
   int8_t w[EM_BUILD], off[EM_BUILD];
   const void* in[EM_BUILD];
 };
-__global__ void __launch_bounds__(256) join_pack_payload_kernel(const __grid_constant__ PackCols pc, int64_t rows, unsigned long long* __restrict__ out) {
-  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < rows; r += (int64_t)gridDim.x * blockDim.x) {
+// packed row i holds build row order[i] (a direct table's rank order), or row i when order is null
+__global__ void __launch_bounds__(256) join_pack_payload_kernel(const __grid_constant__ PackCols pc, int64_t rows, const int32_t* __restrict__ order,
+                                                                unsigned long long* __restrict__ out) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < rows; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = order ? (int64_t)order[i] : i;
     uint64_t lo = 0, hi = 0;
     for (int c = 0; c < pc.n; c++) {
       if (pc.w[c] == 16) { const ulonglong2 v = reinterpret_cast<const ulonglong2*>(pc.in[c])[r]; lo = v.x; hi = v.y; continue; }
@@ -743,12 +834,14 @@ __global__ void __launch_bounds__(256) join_pack_payload_kernel(const __grid_con
                          << (8 * (pc.off[c] & 7));
       if (pc.off[c] & 8) hi |= v; else lo |= v;
     }
-    if (pc.words == 2) reinterpret_cast<ulonglong2*>(out)[r] = make_ulonglong2(lo, hi);
-    else out[r] = lo;
+    if (pc.words == 2) reinterpret_cast<ulonglong2*>(out)[i] = make_ulonglong2(lo, hi);
+    else out[i] = lo;
   }
 }
 
-bool join_pack_payload(const Table* build, const std::vector<int>& cols, JoinPayload& pl) {
+bool join_pack_payload(b2_handle ht, const Table* build, const std::vector<int>& cols, JoinPayload& pl) {
+  const JoinTable* jt = jt_from(ht);
+  if (build->rows != jt->build_rows) throw Error(B2_ERR_INVALID, "join payload table does not match the hash table");
   if (cols.size() > (size_t)EM_BUILD) return false;
   int bytes = 0;
   for (int c : cols) {
@@ -771,10 +864,14 @@ bool join_pack_payload(const Table* build, const std::vector<int>& cols, JoinPay
       pc.w[pc.n] = (int8_t)w; pc.off[pc.n] = (int8_t)at; pc.in[pc.n] = build->cols[cols[k]]->data.p; pc.n++;
       at += w;
     }
-  const int64_t rows = build->rows;
+  // a direct table's probe finds ranks, not rows: its payload is packed in rank order, one row per present key
+  const int64_t rows = jt->direct ? jt->npresent : build->rows;
+  pl.table = ht;
+  pl.rank_order = jt->direct;
   pl.packed = DevBuf(pl.width ? (size_t)rows * pl.width : 0);
   if (pl.width && rows)
-    launch("join_pack_payload_kernel", join_pack_payload_kernel, grid_for(rows, 256), 256, 0, stream(), pc, rows, pl.packed.as<unsigned long long>());
+    launch("join_pack_payload_kernel", join_pack_payload_kernel, grid_for(rows, 256), 256, 0, stream(), pc, rows,
+           jt->direct ? jt->drows.as<int32_t>() : nullptr, pl.packed.as<unsigned long long>());
   return true;
 }
 
@@ -784,7 +881,8 @@ bool join_probe_pred_emit(b2_handle ht, const Table* batch, int key_col, const P
   const Column* pc = nullptr;
   SimplePred sp;
   if (!filter_probe_applies(jt, batch, key_col, prog, pc, sp) || stream_cols.size() > (size_t)EM_STREAM) return false;
-  if (pl.packed.bytes != (size_t)jt->build_rows * pl.width) throw Error(B2_ERR_INVALID, "join payload does not match the hash table");
+  if (pl.table != ht || pl.rank_order != jt->direct || pl.packed.bytes != (size_t)(jt->direct ? jt->npresent : jt->build_rows) * pl.width)
+    throw Error(B2_ERR_INVALID, "join payload does not match the hash table");
   for (int c : stream_cols) {
     if (c < 0 || c >= (int)batch->cols.size()) throw Error(B2_ERR_INVALID, "join column index out of range");
     const Column* ic = batch->cols[c];
@@ -810,15 +908,18 @@ bool join_probe_pred_emit(b2_handle ht, const Table* batch, int key_col, const P
   CUDA_CHECK(cudaMemsetAsync(tot.p, 0, 16, stream()));
   {
     const int grid = grid_for(n, FP_TILE, FP_CTAS);
-    const uint64_t* sl = jt->slots.as<uint64_t>(); const uint32_t msk = (uint32_t)(jt->cap - 1);
-    const unsigned long long* bl = jt->bloom.as<unsigned long long>();
+    const HashView hv = hash_view(jt);
+    const uint64_t* sl = hv.slots; const uint32_t msk = hv.mask;
+    const unsigned long long* bl = hv.bloom;
     unsigned long long* tp = tot.as<unsigned long long>();
+    const DirectMap dm = direct_map(jt);
+    const bool d = jt->direct;
     if (dtype_width(pc->dtype) == 8)
-      launch("join_filter_probe_kernel", join_filter_probe_kernel<int64_t, false, true>, grid, SF_NT, 0, stream(), sp, pc->data.as<int64_t>(), n, sl, msk,
-             bl, jt->bloom_mask, tp, nullptr, nullptr, tp + 1, nullptr, em);
+      launch("join_filter_probe_kernel", d ? join_filter_probe_kernel<int64_t, false, true, true> : join_filter_probe_kernel<int64_t, false, true>, grid,
+             SF_NT, 0, stream(), sp, pc->data.as<int64_t>(), n, sl, msk, bl, hv.bloom_mask, tp, nullptr, nullptr, tp + 1, nullptr, em, dm);
     else
-      launch("join_filter_probe_kernel", join_filter_probe_kernel<int32_t, false, true>, grid, SF_NT, 0, stream(), sp, pc->data.as<int32_t>(), n, sl, msk,
-             bl, jt->bloom_mask, tp, nullptr, nullptr, tp + 1, nullptr, em);
+      launch("join_filter_probe_kernel", d ? join_filter_probe_kernel<int32_t, false, true, true> : join_filter_probe_kernel<int32_t, false, true>, grid,
+             SF_NT, 0, stream(), sp, pc->data.as<int32_t>(), n, sl, msk, bl, hv.bloom_mask, tp, nullptr, nullptr, tp + 1, nullptr, em, dm);
   }
   unsigned long long h[2] = {0, 0};
   d2h(h, tot.p, 2);
@@ -832,29 +933,142 @@ bool join_probe_pred_emit(b2_handle ht, const Table* batch, int key_col, const P
   return true;
 }
 
-}  // namespace b2
+// ---- the direct layout: when a table takes it, and how it is built ----------------------------------------------------------
+// A table with one distinct integer key column goes direct when the span R = max - min + 1 of its non-NULL keys satisfies
+//   R <= DIRECT_MAX_BITS: a bitmap of at most 32 MB, the Bloom filter's cap (a 32 MB Bloom filter was already much slower than a
+//                         16 MB one on the 50 MB L2 of an H100: §9 of DESIGN.md), and ranks that fit a 32-bit offset;
+//   R <= DIRECT_DENSITY x the non-NULL keys: at most 8 B of bitmap, 1 B of block ranks and 4 B of row ids per build row,
+//                         against 32 B per row of hash slots (16-byte slots at load <= 0.5) and 1 B of Bloom filter.
+// The hash table stays for everything else: sparse keys, several or non-integer key columns, duplicate keys.
+constexpr uint64_t DIRECT_MAX_BITS = 1ull << 28, DIRECT_DENSITY = 64;
+__host__ __device__ __forceinline__ bool direct_gate(uint64_t span, uint64_t keys) {   // span = max - min = R - 1
+  return keys > 0 && span < DIRECT_MAX_BITS && span < DIRECT_DENSITY * keys;
+}
+// stats: [0] least key, [1] greatest key (both with the sign bit flipped: ordered as unsigned), [2] non-NULL keys, [3] set when a
+// key was seen twice.  The kernels after the range reduction read the gate from these on the device, so that the layout is
+// chosen without a host round trip before the bitmap is built.
+constexpr unsigned long long KEY_SIGN = 1ull << 63;
+template <typename K>
+__global__ void __launch_bounds__(256) join_key_range_kernel(const K* __restrict__ keys, const uint32_t* __restrict__ valid, int64_t n,
+                                                             unsigned long long* __restrict__ stats) {
+  unsigned long long lo = ~0ull, hi = 0, cnt = 0;
+  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < n; r += (int64_t)gridDim.x * blockDim.x) {
+    if (!row_valid(valid, r)) continue;
+    const unsigned long long u = (uint64_t)(int64_t)keys[r] ^ KEY_SIGN;
+    lo = min(lo, u); hi = max(hi, u); cnt++;
+  }
+  for (int o = 16; o > 0; o >>= 1) {
+    lo = min(lo, __shfl_xor_sync(0xffffffffu, lo, o)); hi = max(hi, __shfl_xor_sync(0xffffffffu, hi, o)); cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+  }
+  if ((threadIdx.x & 31) == 0 && cnt) { atomicMin(&stats[0], lo); atomicMax(&stats[1], hi); atomicAdd(&stats[2], cnt); }
+}
+// zeroes the bitmap the gate admits (`stats` decides; the buffer is allocated for the largest one it could admit)
+__global__ void __launch_bounds__(256) join_direct_clear_kernel(const unsigned long long* __restrict__ stats, unsigned long long* __restrict__ bits) {
+  const uint64_t span = stats[1] - stats[0];
+  if (!direct_gate(span, stats[2])) return;
+  const int64_t words = (int64_t)((span >> 8) + 1) * 4;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < words; i += (int64_t)gridDim.x * blockDim.x) bits[i] = 0;
+}
+// one bit per non-NULL key; a bit that was already set is a duplicate key
+template <typename K>
+__global__ void __launch_bounds__(256) join_direct_build_kernel(const K* __restrict__ keys, const uint32_t* __restrict__ valid, int64_t n,
+                                                                unsigned long long* __restrict__ stats, unsigned long long* __restrict__ bits) {
+  const uint64_t span = stats[1] - stats[0], lo = stats[0] ^ KEY_SIGN;
+  if (!direct_gate(span, stats[2])) return;
+  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < n; r += (int64_t)gridDim.x * blockDim.x) {
+    if (!row_valid(valid, r)) continue;
+    const uint64_t o = (uint64_t)(int64_t)keys[r] - lo;
+    const unsigned long long b = 1ull << (o & 63);
+    if (atomicOr(&bits[o >> 6], b) & b) stats[3] = 1;
+  }
+}
+// keys per 256-bit block (then exclusive_scan: the block ranks)
+__global__ void __launch_bounds__(256) join_direct_count_kernel(const ulonglong2* __restrict__ bits, int64_t nblocks, uint32_t* __restrict__ counts) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < nblocks; i += (int64_t)gridDim.x * blockDim.x) {
+    const ulonglong2 a = bits[2 * i], c = bits[2 * i + 1];
+    counts[i] = (uint32_t)(__popcll(a.x) + __popcll(a.y) + __popcll(c.x) + __popcll(c.y));
+  }
+}
+// rows[rank of the key of build row r] = r
+template <typename K>
+__global__ void __launch_bounds__(256) join_direct_rows_kernel(const K* __restrict__ keys, const uint32_t* __restrict__ valid, int64_t n,
+                                                               const __grid_constant__ DirectMap dm, int32_t* __restrict__ rows) {
+  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < n; r += (int64_t)gridDim.x * blockDim.x) {
+    if (!row_valid(valid, r)) continue;
+    rows[direct_rank(dm, direct_off(dm, keys[r]))] = (int32_t)r;
+  }
+}
 
-using namespace b2;
-extern "C" {
+// whether jt's one key column may go direct: a fast table (no NULL can match) of one 4- or 8-byte integer-like key column
+static bool direct_candidate(const JoinTable* jt) {
+  const Table* t = jt->keys;
+  if (!jt->fast || t->cols.size() != 1 || t->rows == 0 || t->rows >= 0x7fffffffLL || getenv("B2_JOIN_NO_DIRECT")) return false;
+  switch (t->cols[0]->dtype) {
+    case B2_INT32: case B2_DATE32: case B2_DECIMAL32: case B2_INT64: case B2_TIMESTAMP_US: case B2_DECIMAL64: return true;
+    default: return false;
+  }
+}
+template <typename K>
+static void direct_build_launch(const Column* kc, int64_t n, unsigned long long* stats, DevBuf& bits) {
+  const K* keys = kc->data.as<K>();
+  launch("join_key_range_kernel", join_key_range_kernel<K>, grid_for(n, 256), 256, 0, stream(), keys, kc->validity(), n, stats);
+  launch("join_direct_clear_kernel", join_direct_clear_kernel, grid_for((int64_t)(bits.bytes / 8), 256), 256, 0, stream(), stats, bits.as<unsigned long long>());
+  launch("join_direct_build_kernel", join_direct_build_kernel<K>, grid_for(n, 256), 256, 0, stream(), keys, kc->validity(), n, stats, bits.as<unsigned long long>());
+}
+template <typename K>
+static void direct_rows_launch(JoinTable* jt) {
+  const Column* kc = jt->keys->cols[0];
+  launch("join_direct_rows_kernel", join_direct_rows_kernel<K>, grid_for(jt->build_rows, 256), 256, 0, stream(), kc->data.as<K>(), kc->validity(),
+         jt->build_rows, direct_map(jt), jt->drows.as<int32_t>());
+}
+// Builds jt's direct layout when the gate admits it and no key repeats.  One host round trip, the one a hash build takes for its
+// duplicate flag.  False: nothing kept, build the hash table (which takes its own round trip: to fold the two, the hash table
+// would have to be allocated and cleared before the layout is known, the 32 B per row a direct table saves).
+static bool direct_build(JoinTable* jt) {
+  const Column* kc = jt->keys->cols[0];
+  const int64_t n = jt->build_rows;
+  const bool wide = dtype_width(kc->dtype) == 8;
+  DevBuf stats(32);
+  CUDA_CHECK(cudaMemsetAsync(stats.p, 0xff, 8, stream()));
+  CUDA_CHECK(cudaMemsetAsync(stats.as<unsigned long long>() + 1, 0, 24, stream()));
+  const uint64_t most = std::min<uint64_t>(DIRECT_MAX_BITS, DIRECT_DENSITY * (uint64_t)n);   // the largest span the gate admits
+  DevBuf bits((size_t)((most + 255) / 256) * 32);
+  if (wide) direct_build_launch<int64_t>(kc, n, stats.as<unsigned long long>(), bits);
+  else direct_build_launch<int32_t>(kc, n, stats.as<unsigned long long>(), bits);
+  unsigned long long h[4];
+  d2h(h, stats.p, 4);
+  sync();
+  const uint64_t span = h[1] - h[0];
+  if (!direct_gate(span, h[2]) || h[3]) return false;
+  jt->direct = true;
+  jt->distinct = true;
+  jt->dlo = (int64_t)(h[0] ^ KEY_SIGN);
+  jt->drange = span + 1;
+  jt->npresent = (int64_t)h[2];
+  const int64_t nblocks = (int64_t)((jt->drange + 255) / 256);
+  // the scratch was sized for the largest span the gate admits (min(2^28, 64 x rows) bits: up to 32 MB); the table keeps only
+  // the blocks of its own span (q3: 1.9 of 24 MB for customer, 18.75 of 32 MB for orders), one device copy
+  jt->dbits = DevBuf((size_t)nblocks * 32);
+  CUDA_CHECK(cudaMemcpyAsync(jt->dbits.p, bits.p, jt->dbits.bytes, cudaMemcpyDeviceToDevice, stream()));
+  bits.reset();   // stream-ordered free, after the copy
+  jt->dranks = DevBuf((size_t)(nblocks + 1) * 4);
+  launch("join_direct_count_kernel", join_direct_count_kernel, grid_for(nblocks, 256), 256, 0, stream(), jt->dbits.as<ulonglong2>(), nblocks,
+         jt->dranks.as<uint32_t>());
+  exclusive_scan<uint32_t, uint32_t>(jt->dranks.as<uint32_t>(), jt->dranks.as<uint32_t>(), nblocks, true);
+  jt->drows = DevBuf((size_t)jt->npresent * 4);
+  if (wide) direct_rows_launch<int64_t>(jt);
+  else direct_rows_launch<int32_t>(jt);
+  return true;
+}
 
-int b2_join_build(b2_handle build_keys_table, int32_t nulls_equal, b2_handle* out_hash_table) {
-  B2_TRY
-  Table* t = table_from(build_keys_table);
-  B2_CHECK(!t->cols.empty() && (int)t->cols.size() <= MAX_KEYS, "join needs 1..8 key columns");
-  std::unique_ptr<JoinTable> jt(new JoinTable());
-  t->refs.fetch_add(1);
-  jt->keys = t;
-  jt->build_rows = t->rows;
-  jt->nulls_equal = nulls_equal != 0;
-  for (int i = 0; i < (int)t->cols.size(); i++) jt->key_idx.push_back(i);
+// The open-addressing table (and Bloom filter) over jt->keys; returns whether no key repeats.  b2_join_build builds it for every
+// table that does not go direct; a direct table builds it through ensure_hash on the first probe that needs it (SEMI / ANTI,
+// LEFT OUTER, a nullable probe key).
+static bool hash_build(JoinTable* jt) {
+  Table* t = jt->keys;
   int64_t cap = 1024;
   while (cap < t->rows * 2) cap <<= 1;
   jt->cap = cap;
-  {
-    int kw = 0; bool fixed = true, nullable = false;
-    for (auto* c : t->cols) { if (c->dtype == B2_STRING || c->dtype == B2_DECIMAL128) fixed = false; kw += dtype_width(c->dtype); nullable = nullable || c->nullable(); }
-    jt->fast = fixed && kw <= 8 && !(jt->nulls_equal && nullable);
-  }
   jt->slots = DevBuf((size_t)cap * (jt->fast ? 16 : 8));
   CUDA_CHECK(cudaMemsetAsync(jt->slots.p, 0xff, jt->slots.bytes, stream()));
   if (t->rows >= (1 << 18) && !getenv("B2_JOIN_NO_BLOOM")) {   // smaller tables are L2 resident themselves
@@ -883,7 +1097,38 @@ int b2_join_build(b2_handle build_keys_table, int32_t nulls_equal, b2_handle* ou
   int32_t h_dups = 0;
   d2h(&h_dups, dups.p, 1);
   sync();
-  jt->distinct = h_dups == 0;
+  jt->hashed.store(true, std::memory_order_release);   // after sync(): complete for every stream
+  return h_dups == 0;
+}
+// the hash table of a direct table, built once whichever task thread asks first; the others wait for it
+static void ensure_hash(JoinTable* jt) {
+  if (jt->hashed.load(std::memory_order_acquire)) return;
+  std::lock_guard<std::mutex> lk(jt->hash_mu);
+  if (!jt->hashed.load(std::memory_order_relaxed)) hash_build(jt);   // distinct already known: the direct build found no repeat
+}
+
+}  // namespace b2
+
+using namespace b2;
+extern "C" {
+
+int b2_join_build(b2_handle build_keys_table, int32_t nulls_equal, b2_handle* out_hash_table) {
+  B2_TRY
+  Table* t = table_from(build_keys_table);
+  B2_CHECK(!t->cols.empty() && (int)t->cols.size() <= MAX_KEYS, "join needs 1..8 key columns");
+  std::unique_ptr<JoinTable> jt(new JoinTable());
+  t->refs.fetch_add(1);
+  jt->keys = t;
+  jt->build_rows = t->rows;
+  jt->nulls_equal = nulls_equal != 0;
+  for (int i = 0; i < (int)t->cols.size(); i++) jt->key_idx.push_back(i);
+  {
+    int kw = 0; bool fixed = true, nullable = false;
+    for (auto* c : t->cols) { if (c->dtype == B2_STRING || c->dtype == B2_DECIMAL128) fixed = false; kw += dtype_width(c->dtype); nullable = nullable || c->nullable(); }
+    jt->fast = fixed && kw <= 8 && !(jt->nulls_equal && nullable);
+  }
+  // dense distinct integer keys: the direct layout (no hash, no slots, no Bloom filter); otherwise the hash table
+  if (!(direct_candidate(jt.get()) && direct_build(jt.get()))) jt->distinct = hash_build(jt.get());
   *out_hash_table = to_handle(jt.release());
   B2_CATCH
 }
@@ -943,6 +1188,13 @@ static void probe_maps(JoinTable* jt, Table* pt, b2_handle selection, int32_t ki
   const bool semi_like = kind == B2_JOIN_LEFT_SEMI || kind == B2_JOIN_LEFT_ANTI;
   KeyCols pk = key_cols_of(pt, jt->key_idx.data(), (int)jt->key_idx.size());
   KeyCols bk = key_cols_of(jt->keys, jt->key_idx.data(), (int)jt->key_idx.size());
+  const Column* pc = jt->key_idx.size() == 1 ? pt->cols[jt->key_idx[0]] : nullptr;
+  const int pw = pc ? dtype_width(pc->dtype) : 0;
+  // the one-key probe (join_probe_distinct1_kernel), the only one with a direct variant: every other probe of a direct table
+  // builds its hash table first
+  const bool one_key = jt->distinct && kind == B2_JOIN_INNER && jt->fast && pc && !pc->nullable() && !is_float(pc->dtype) && pc->dtype != B2_STRING &&
+                       (pw == 4 || pw == 8) && n < 0x7fffffffLL && !getenv("B2_JOIN_NO_FAST_PROBE");
+  if (n && !(one_key && jt->direct)) ensure_hash(jt);
   if (jt->distinct && (kind == B2_JOIN_INNER || kind == B2_JOIN_LEFT_OUTER)) {
     // innerDistinctJoinGatherMaps / leftDistinctJoinGatherMap fast path (GpuHashJoin.scala:1401-1428)
     ColGuard lm(new_column(B2_INT32, 0, n, false)), rm(new_column(B2_INT32, 0, n, false));
@@ -950,28 +1202,36 @@ static void probe_maps(JoinTable* jt, Table* pt, b2_handle selection, int32_t ki
     if (n) {
       DevBuf tot(8);
       CUDA_CHECK(cudaMemsetAsync(tot.p, 0, 8, stream()));
-      L2Persist keep(jt->bloom.p, jt->bloom.bytes);
-      const Column* pc = jt->key_idx.size() == 1 ? pt->cols[jt->key_idx[0]] : nullptr;
-      const int pw = pc ? dtype_width(pc->dtype) : 0;
-      if (kind == B2_JOIN_INNER && jt->fast && pc && !pc->nullable() && !is_float(pc->dtype) && pc->dtype != B2_STRING && (pw == 4 || pw == 8) &&
-          n < 0x7fffffffLL && !getenv("B2_JOIN_NO_FAST_PROBE")) {
+      L2Persist keep(jt->direct && one_key ? nullptr : jt->bloom.p, jt->direct && one_key ? 0 : jt->bloom.bytes);
+      if (one_key) {
         const int grid = grid_for(n, 256);
-        const uint64_t* sl = jt->slots.as<uint64_t>(); const uint32_t msk = (uint32_t)(jt->cap - 1);
-        const unsigned long long* bl = jt->bloom.as<unsigned long long>(); unsigned long long* tp = tot.as<unsigned long long>();
+        const HashView hv = hash_view(jt);
+        const uint64_t* sl = hv.slots; const uint32_t msk = hv.mask;
+        const unsigned long long* bl = hv.bloom; unsigned long long* tp = tot.as<unsigned long long>();
         int32_t* lp = lm.c->data.as<int32_t>(); int32_t* rp = rm.c->data.as<int32_t>();
+        const DirectMap dm = direct_map(jt);
+        const bool d = jt->direct;
         if (track) {
           if (pw == 8)
-            launch("join_probe_distinct1_track_kernel", sel ? join_probe_distinct1_kernel<int64_t, true, true> : join_probe_distinct1_kernel<int64_t, false, true>,
-                   grid, 256, 0, stream(), pc->data.as<int64_t>(), sel, n, sl, msk, bl, jt->bloom_mask, tp, lp, rp, track);
+            launch("join_probe_distinct1_track_kernel",
+                   d ? (sel ? join_probe_distinct1_kernel<int64_t, true, true, true> : join_probe_distinct1_kernel<int64_t, false, true, true>)
+                     : (sel ? join_probe_distinct1_kernel<int64_t, true, true> : join_probe_distinct1_kernel<int64_t, false, true>),
+                   grid, 256, 0, stream(), pc->data.as<int64_t>(), sel, n, sl, msk, bl, hv.bloom_mask, tp, lp, rp, track, dm);
           else
-            launch("join_probe_distinct1_track_kernel", sel ? join_probe_distinct1_kernel<int32_t, true, true> : join_probe_distinct1_kernel<int32_t, false, true>,
-                   grid, 256, 0, stream(), pc->data.as<int32_t>(), sel, n, sl, msk, bl, jt->bloom_mask, tp, lp, rp, track);
+            launch("join_probe_distinct1_track_kernel",
+                   d ? (sel ? join_probe_distinct1_kernel<int32_t, true, true, true> : join_probe_distinct1_kernel<int32_t, false, true, true>)
+                     : (sel ? join_probe_distinct1_kernel<int32_t, true, true> : join_probe_distinct1_kernel<int32_t, false, true>),
+                   grid, 256, 0, stream(), pc->data.as<int32_t>(), sel, n, sl, msk, bl, hv.bloom_mask, tp, lp, rp, track, dm);
         } else if (pw == 8) {
-          launch("join_probe_distinct1_kernel", sel ? join_probe_distinct1_kernel<int64_t, true, false> : join_probe_distinct1_kernel<int64_t, false, false>,
-                 grid, 256, 0, stream(), pc->data.as<int64_t>(), sel, n, sl, msk, bl, jt->bloom_mask, tp, lp, rp, nullptr);
+          launch("join_probe_distinct1_kernel",
+                 d ? (sel ? join_probe_distinct1_kernel<int64_t, true, false, true> : join_probe_distinct1_kernel<int64_t, false, false, true>)
+                   : (sel ? join_probe_distinct1_kernel<int64_t, true, false> : join_probe_distinct1_kernel<int64_t, false, false>),
+                 grid, 256, 0, stream(), pc->data.as<int64_t>(), sel, n, sl, msk, bl, hv.bloom_mask, tp, lp, rp, nullptr, dm);
         } else {
-          launch("join_probe_distinct1_kernel", sel ? join_probe_distinct1_kernel<int32_t, true, false> : join_probe_distinct1_kernel<int32_t, false, false>,
-                 grid, 256, 0, stream(), pc->data.as<int32_t>(), sel, n, sl, msk, bl, jt->bloom_mask, tp, lp, rp, nullptr);
+          launch("join_probe_distinct1_kernel",
+                 d ? (sel ? join_probe_distinct1_kernel<int32_t, true, false, true> : join_probe_distinct1_kernel<int32_t, false, false, true>)
+                   : (sel ? join_probe_distinct1_kernel<int32_t, true, false> : join_probe_distinct1_kernel<int32_t, false, false>),
+                 grid, 256, 0, stream(), pc->data.as<int32_t>(), sel, n, sl, msk, bl, hv.bloom_mask, tp, lp, rp, nullptr, dm);
         }
       } else {
         launch(track ? "join_probe_distinct_track_kernel" : "join_probe_distinct_kernel",
