@@ -429,12 +429,30 @@ int b2_broadcast_table(b2_handle comm, b2_handle table, int32_t root, b2_handle*
  *   column's type, b2_groupby's order (NaN greatest); STRING and DECIMAL128: B2_ERR_UNSUPPORTED.  SUM, MIN, MAX are NULL on an
  *   empty or all-NULL frame.  Frames: ROWS [lower, upper] (row offsets, 0 = CURRENT ROW, or the UNBOUNDED sentinels, clipped to
  *   the partition); RANGE only UNBOUNDED PRECEDING -> CURRENT ROW (to the end of the peer group) or -> UNBOUNDED FOLLOWING
- *   (value offsets: B2_ERR_UNSUPPORTED).  A float SUM is a parallel scan: it may differ from a left-to-right sum in the last bits. */
+ *   (value offsets: B2_ERR_UNSUPPORTED); RANGE_VALUE below.  A float SUM is a parallel scan or a range query over partial
+ *   sums: it may differ from a left-to-right sum in the last bits, and is exact where every partial sum is exact in double.
+ * RANGE_VALUE [lower, upper] (Spark's RangeBoundOrdering; BasicWindowCalc.scala:169-219): value offsets in the units of the
+ *   ORDER BY column (integers: values; DATE32: days; TIMESTAMP_US: microseconds; DECIMAL32/64/128: unscaled values at the
+ *   column's scale), 0 = CURRENT ROW (the edge of the row's peer group), the UNBOUNDED sentinels = the partition's edge.  For a
+ *   row with ORDER BY value v the bound values are v + lower and v + upper (ASC) or v - lower and v - upper (DESC), exact in
+ *   128 bits, so they never wrap (Spark's CPU wraps integral bounds); NULL when v is NULL.  The frame [s, e] is, within the
+ *   partition, s = the first row whose value is >= the lower bound value in the sort order and e = the last row whose value is
+ *   <= the upper one (NULL = NULL, NULLs sort where nulls_first puts them, DESC reverses the comparison); s > e: empty.  So a
+ *   NULL row's frame is its NULL peer group, widened to the partition edge on an UNBOUNDED side; a non-NULL row's bounded frame
+ *   never holds a NULL row, while a frame to UNBOUNDED FOLLOWING holds the trailing NULLs of nulls last.  Offsets may have
+ *   either sign (1 FOLLOWING -> 3 FOLLOWING is [1, 3]).  A decimal SUM is NULL when the frame's total does not fit.
+ *   (UNBOUNDED, 0) is RANGE's running frame (its sticky decimal overflow included) and (UNBOUNDED, UNBOUNDED) the whole
+ *   partition: both run exactly as B2_FRAME_RANGE does.  Other frames: a binary search per row and bound in the partition,
+ *   once per distinct (lower, upper); SUM of integers and decimals and COUNT are a difference of prefixes, float SUM / MIN /
+ *   MAX a range query whose work per row does not grow with the frame (32 B per row of device memory per such function for
+ *   its 16-byte state).  Bounds of only 0 and UNBOUNDED need peer groups only and take any ORDER BY.  Errors, B2_ERR_INVALID:
+ *   no ORDER BY with a bound other than UNBOUNDED; lower > upper or a bound in the wrong direction; a value offset with more
+ *   than one ORDER BY column or over a STRING or BOOL8 one.  B2_ERR_UNSUPPORTED: a value offset over FLOAT32 / FLOAT64. */
 typedef enum {
   B2_WIN_ROW_NUMBER = 1, B2_WIN_RANK = 2, B2_WIN_DENSE_RANK = 3, B2_WIN_LEAD = 4, B2_WIN_LAG = 5,
   B2_WIN_SUM = 10, B2_WIN_COUNT = 11, B2_WIN_COUNT_ALL = 12, B2_WIN_MIN = 13, B2_WIN_MAX = 14
 } b2_window_kind;
-typedef enum { B2_FRAME_ROWS = 0, B2_FRAME_RANGE = 1 } b2_frame_type;
+typedef enum { B2_FRAME_ROWS = 0, B2_FRAME_RANGE = 1, B2_FRAME_RANGE_VALUE = 2 } b2_frame_type;
 #define B2_UNBOUNDED_PRECEDING INT64_MIN
 #define B2_UNBOUNDED_FOLLOWING INT64_MAX
 typedef struct {
@@ -544,7 +562,8 @@ int b2_exec_coalesce(b2_handle child, int64_t target_rows, b2_handle* out);     
  *     rows of context; neither the input nor a partition has to fit on the device, and the input may pass 2^31 rows.  A batch
  *     plus P + F rows of 2^31 or more: B2_ERR_SIZE_OVERFLOW.
  *   Held: any other plan.  With RANGE running frames beside running functions only, each batch's trailing peer group waits
- *     for the next batch; otherwise (a frame to UNBOUNDED FOLLOWING, or a bounded function beside a RANGE frame) the trailing
+ *     for the next batch; otherwise (a frame to UNBOUNDED FOLLOWING, a RANGE_VALUE frame other than the running one, or a
+ *     bounded function beside a RANGE frame) the trailing
  *     partition waits (no PARTITION BY: the whole input is one group).  Waiting rows are held in the spill store and concatenated when their group
  *     ends; a group of 2^31-1 rows or more: B2_ERR_SIZE_OVERFLOW.
  * Running and bounded: an allocation failure halves a batch, and each half becomes an output batch. */

@@ -27,7 +27,7 @@ AGG_SUM, AGG_COUNT, AGG_MIN, AGG_MAX, AGG_COUNT_ALL = 1, 2, 3, 4, 5
 # b2_window_kind, b2_frame_type
 WIN_ROW_NUMBER, WIN_RANK, WIN_DENSE_RANK, WIN_LEAD, WIN_LAG = 1, 2, 3, 4, 5
 WIN_SUM, WIN_COUNT, WIN_COUNT_ALL, WIN_MIN, WIN_MAX = 10, 11, 12, 13, 14
-FRAME_ROWS, FRAME_RANGE = 0, 1
+FRAME_ROWS, FRAME_RANGE, FRAME_RANGE_VALUE = 0, 1, 2
 UNBOUNDED_PRECEDING, UNBOUNDED_FOLLOWING = -2**63, 2**63 - 1
 # b2_join_kind
 JOIN_INNER, JOIN_LEFT_OUTER, JOIN_LEFT_SEMI, JOIN_LEFT_ANTI, JOIN_FULL_OUTER, JOIN_RIGHT_OUTER = 0, 1, 2, 3, 4, 5
@@ -415,7 +415,10 @@ def _order_args(keys):
 
 
 class Frame:
-    """a window frame: ROWS or RANGE, bounds as row offsets (0 = CURRENT ROW, None = UNBOUNDED)"""
+    """a window frame: its type and its bounds, with 0 = CURRENT ROW and None = UNBOUNDED PRECEDING (lower) / FOLLOWING (upper).
+    FRAME_ROWS: bounds are row offsets.  FRAME_RANGE: only (None, 0) and (None, None).  FRAME_RANGE_VALUE: bounds are value
+    offsets in the units of the single ORDER BY column (integers: values; DATE32: days; TIMESTAMP_US: microseconds; decimals:
+    unscaled values at the column's scale), subtracted instead of added under a descending order; 0 is the peer group's edge"""
 
     def __init__(self, frame_type, lower, upper):
         self.type, self.lower, self.upper = frame_type, lower, upper
@@ -429,6 +432,12 @@ def rows(lower, upper):
 def range_running():
     """RANGE BETWEEN UNBOUNDED PRECEDING AND CURRENT ROW: Spark's default frame with ORDER BY"""
     return Frame(FRAME_RANGE, None, 0)
+
+
+def range_between(lower, upper):
+    """RANGE BETWEEN lower AND upper by value (None = UNBOUNDED PRECEDING / FOLLOWING, 0 = CURRENT ROW), e.g. 7 days before a
+    DATE32 row up to it: range_between(-7, 0)"""
+    return Frame(FRAME_RANGE_VALUE, lower, upper)
 
 
 def unbounded():

@@ -1414,7 +1414,8 @@ struct GpuOutOfCoreSortExec : GpuExec {
 //      its own rows are written, and the output batch is its own columns (by reference) and the function columns.  The carry is
 //      taken at the row before the next chunk's first row.  An OOM splits the batch in halves, each run with its own context;
 //   2. a RANGE running frame: the trailing peer group of each batch waits for the next (BatchedByKey(partition ++ order));
-//   3. a frame to the partition's end, or a bounded frame or LEAD / LAG beside a RANGE frame: the trailing partition waits
+//   3. a frame to the partition's end, a RANGE frame with value offsets, or a bounded frame or LEAD / LAG beside a RANGE frame:
+//      the trailing partition waits
 //      (BatchedByKey(partition); with no PARTITION BY the whole input is one group, RequireSingleBatch).
 // Waiting rows of modes 2 and 3 are pieces in the spill store, concatenated once when their group ends; finding the group end of a
 // batch costs one device-to-host copy of an index.

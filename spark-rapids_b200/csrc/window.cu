@@ -18,6 +18,15 @@
 //   window_lead_lag_kernel    LEAD / LAG source row (or -1 outside the partition); values through gather_table, then the default
 // Finish and LEAD / LAG run over every row of the chunk (AllRows) or, for a streamed bounded plan, only over the rows [lo, hi)
 // between its context and look-ahead rows (RowRange), writing columns of hi - lo rows.
+// RANGE frames with value offsets (B2_FRAME_RANGE_VALUE; BasicWindowCalc.scala:169-219, 445 aggregateWindowsOverRanges):
+//   window_range_bounds_kernel  each row's frame [s, e], once per distinct (lower, upper): a binary search of the ORDER BY
+//                               values in the partition for a value offset, the peer-group or partition edge otherwise
+//   window_range_tiles_kernel   non-SUB ops (float SUM, MIN, MAX): per WIN_TILE-row tile the unsegmented in-tile prefix and
+//                               suffix of the state and the tile's aggregate
+//   window_range_table_kernel   one level of a sparse table over the tile aggregates (level k: tiles [t, t + 2^k))
+//   window_range_finish_kernel  the frame's value: state[e] from the partition start, a difference of prefixes for SUB ops,
+//                               otherwise suffix[s] + O(log tiles) levels + prefix[e] (a loop when s and e share a tile), so
+//                               the work per row is bounded by WIN_TILE + log2(tiles) whatever the frame's width
 #include <algorithm>
 #include "sortkey.cuh"
 #include "window.cuh"
@@ -349,7 +358,7 @@ __global__ void __launch_bounds__(WIN_NT) window_scan_kernel(const Op op, const 
 
 // ------------------------------------------------------------------------------------------------
 // frames
-enum { FR_ROWS_RUNNING = 0, FR_RANGE_RUNNING = 1, FR_GENERAL = 2 };
+enum { FR_ROWS_RUNNING = 0, FR_RANGE_RUNNING = 1, FR_GENERAL = 2, FR_RANGE_VALUE = 3 };
 struct FrameArgs {
   int32_t type, lower_unb, upper_unb;
   int64_t lower, upper;
@@ -441,10 +450,173 @@ __global__ void window_default_kernel(const int32_t* __restrict__ map, int64_t n
 }
 
 // ------------------------------------------------------------------------------------------------
+// RANGE frames with value offsets (Spark's RangeBoundOrdering)
+
+// The first ORDER BY column as a key that ascends in the sort order: x, or -x for DESC, exact in 128 bits, so that the bound
+// values key(i) + lower and key(i) + upper never wrap (|x| < 10^38 for decimals, offsets are int64).  A NULL sorts before every
+// value (nulls first) or after it.  col.data == null: no value offsets, every bounded side is a peer-group edge.
+struct RangeKey {
+  ColView col;
+  int32_t desc, nulls_first;
+  __device__ __forceinline__ i128 at(int64_t j) const {
+    const i128 x = col.width == 16 ? reinterpret_cast<const i128*>(col.data)[j] : (i128)load_int(col, j);
+    return desc ? -x : x;
+  }
+  // the first row j of [lo, hi] whose key is >= b (strict: > b), or hi + 1; the keys of [lo, hi] ascend
+  __device__ int64_t first_past(int64_t lo, int64_t hi, i128 b, bool strict) const {
+    int64_t a = lo, z = hi + 1;
+    while (a < z) {
+      const int64_t mid = a + ((z - a) >> 1);
+      bool past;
+      if (!row_valid(col.valid, mid)) past = !nulls_first;
+      else {
+        const i128 k = at(mid);
+        past = strict ? k > b : k >= b;
+      }
+      if (past) z = mid;
+      else a = mid + 1;
+    }
+    return a;
+  }
+};
+struct RangeBounds {
+  int64_t lower, upper;   // value offsets; 0 = the peer-group edge
+  int32_t lower_unb, upper_unb;
+};
+
+// s[i], e[i]: row i's frame, partition rows only (s > e: empty).  A NULL ORDER BY value's bounds are NULL, so its bounded sides
+// are the edges of its (NULL) peer group; a non-NULL value's bounded frame never reaches a NULL row.
+__global__ void window_range_bounds_kernel(const RangeKey key, const RangeBounds b, const Groups g, int64_t n, int32_t* __restrict__ s_at,
+                                           int32_t* __restrict__ e_at) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const RankOp::T r = g.rank[i];
+    const int64_t ps = max((int64_t)0, i - r.rn + 1), pe = g.pend_at[ps];
+    const int64_t qs = max((int64_t)0, i - r.rn + r.rk), qe = g.peer_end_at[qs];
+    const bool by_peer = key.col.data == nullptr || !row_valid(key.col.valid, i);
+    const i128 v = by_peer ? (i128)0 : key.at(i);
+    int64_t s, e;
+    if (b.lower_unb) s = ps;
+    else if (b.lower == 0 || by_peer) s = qs;
+    else s = key.first_past(ps, pe, v + (i128)b.lower, false);
+    if (b.upper_unb) e = pe;
+    else if (b.upper == 0 || by_peer) e = qe;
+    else e = key.first_past(ps, pe, v + (i128)b.upper, true) - 1;
+    s_at[i] = (int32_t)s;
+    e_at[i] = (int32_t)e;
+  }
+}
+
+// the range-query structure of a non-SUB op over a chunk (unsegmented: a frame never leaves its partition)
+template <typename T>
+struct RangeTable {
+  const T* pre;      // pre[i]: rows [tile start, i]
+  const T* suf;      // suf[i]: rows [i, tile end]
+  const T* levels;   // levels[k * ntiles + t]: tiles [t, t + 2^k)
+  int64_t ntiles;
+  int32_t nlevels;
+};
+
+template <class Op>
+__global__ void __launch_bounds__(WIN_NT) window_range_tiles_kernel(const Op op, int64_t n, typename Op::T* __restrict__ pre, typename Op::T* __restrict__ suf,
+                                                                    typename Op::T* __restrict__ agg) {
+  using T = typename Op::T;
+  __shared__ T s_scan[2][WIN_NT];
+  const int64_t ntiles = (n + WIN_TILE - 1) / WIN_TILE;
+  const int tx = threadIdx.x;
+  for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    const int64_t base = tile * WIN_TILE + (int64_t)tx * WIN_ITEMS;
+    T a = op.identity();
+#pragma unroll
+    for (int k = 0; k < WIN_ITEMS; k++)
+      if (base + k < n) a = op.combine(a, op.elem(base + k));
+    // prefix: inclusive scan of the thread aggregates from the left
+    int cur = 0;
+    s_scan[0][tx] = a;
+    __syncthreads();
+    for (int off = 1; off < WIN_NT; off <<= 1) {
+      T y = s_scan[cur][tx];
+      if (tx >= off) y = op.combine(s_scan[cur][tx - off], y);
+      s_scan[cur ^ 1][tx] = y;
+      cur ^= 1;
+      __syncthreads();
+    }
+    T run = tx > 0 ? s_scan[cur][tx - 1] : op.identity();
+    if (tx == WIN_NT - 1) agg[tile] = s_scan[cur][tx];
+#pragma unroll
+    for (int k = 0; k < WIN_ITEMS; k++)
+      if (base + k < n) { run = op.combine(run, op.elem(base + k)); pre[base + k] = run; }
+    __syncthreads();
+    // suffix: the same from the right
+    cur = 0;
+    s_scan[0][tx] = a;
+    __syncthreads();
+    for (int off = 1; off < WIN_NT; off <<= 1) {
+      T y = s_scan[cur][tx];
+      if (tx + off < WIN_NT) y = op.combine(y, s_scan[cur][tx + off]);
+      s_scan[cur ^ 1][tx] = y;
+      cur ^= 1;
+      __syncthreads();
+    }
+    run = tx < WIN_NT - 1 ? s_scan[cur][tx + 1] : op.identity();
+#pragma unroll
+    for (int k = WIN_ITEMS - 1; k >= 0; k--)
+      if (base + k < n) { run = op.combine(op.elem(base + k), run); suf[base + k] = run; }
+    __syncthreads();
+  }
+}
+
+// level k of the sparse table from level k - 1 (half = 2^(k-1)); entries that would pass the last tile are never read
+template <class Op>
+__global__ void window_range_table_kernel(const Op op, int64_t ntiles, int64_t half, const typename Op::T* __restrict__ prev,
+                                          typename Op::T* __restrict__ next) {
+  for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < ntiles; t += (int64_t)gridDim.x * blockDim.x)
+    next[t] = t + half < ntiles ? op.combine(prev[t], prev[t + half]) : prev[t];
+}
+
+// the op over rows [s, e] (s <= e) through the structure: at most WIN_TILE elements, or two reads and one per level
+template <class Op>
+__device__ __forceinline__ typename Op::T range_query(const Op& op, const RangeTable<typename Op::T>& rt, int64_t s, int64_t e) {
+  using T = typename Op::T;
+  const int64_t ts = s / WIN_TILE, te = e / WIN_TILE;
+  if (ts == te) {
+    T v = op.identity();
+    for (int64_t j = s; j <= e; j++) v = op.combine(v, op.elem(j));
+    return v;
+  }
+  // the whole tiles [ts + 1, te) in blocks of decreasing powers of two, each level at most once
+  T v = rt.suf[s];
+  int64_t a = ts + 1;
+  for (int k = rt.nlevels - 1; k >= 0; k--)
+    if (a + ((int64_t)1 << k) <= te) {
+      v = op.combine(v, rt.levels[(int64_t)k * rt.ntiles + a]);
+      a += (int64_t)1 << k;
+    }
+  return op.combine(v, rt.pre[e]);
+}
+
+// Every row of a chunk that starts at a partition start (a RANGE_VALUE plan holds whole partitions), from s[i] and e[i]
+template <class Op>
+__global__ void window_range_finish_kernel(const Op op, const Groups g, const int32_t* __restrict__ s_at, const int32_t* __restrict__ e_at,
+                                           const typename Op::T* __restrict__ state, const RangeTable<typename Op::T> rt, int64_t n, const WinOut out) {
+  using T = typename Op::T;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t ps = max((int64_t)0, i - g.rank[i].rn + 1), s = s_at[i], e = e_at[i];
+    T v;
+    if (s > e) v = op.identity();
+    else if (s == ps) v = state[e];
+    else if (Op::SUB) v = op.sub(state[e], state[s - 1]);
+    else v = range_query(op, rt, s, e);
+    op.finish(v, false, out, i);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
 // host side
 static bool is_ranking(int k) { return k == B2_WIN_ROW_NUMBER || k == B2_WIN_RANK || k == B2_WIN_DENSE_RANK; }
 static bool is_offset_fn(int k) { return k == B2_WIN_LEAD || k == B2_WIN_LAG; }
 static bool needs_column(int k) { return !is_ranking(k) && k != B2_WIN_COUNT_ALL; }
+// a RANGE_VALUE bound that is a value offset (not CURRENT ROW, not UNBOUNDED)
+static bool value_offset(int64_t b) { return b != 0 && b != B2_UNBOUNDED_PRECEDING && b != B2_UNBOUNDED_FOLLOWING; }
 
 // checks what the specs say about themselves and classifies the frames; column types are checked by bind()
 WindowPlan make_window_plan(const int32_t* part_cols, int nparts, const b2_order_by_arg* order, int norder, const b2_window_spec* specs, int nspecs) {
@@ -471,17 +643,23 @@ WindowPlan make_window_plan(const int32_t* part_cols, int nparts, const b2_order
       }
     } else if (kind == B2_WIN_SUM || kind == B2_WIN_COUNT || kind == B2_WIN_COUNT_ALL || kind == B2_WIN_MIN || kind == B2_WIN_MAX) {
       const bool lu = f.s.lower == B2_UNBOUNDED_PRECEDING, uu = f.s.upper == B2_UNBOUNDED_FOLLOWING;
-      B2_CHECK(f.s.frame == B2_FRAME_ROWS || f.s.frame == B2_FRAME_RANGE, "window: unknown frame type");
+      B2_CHECK(f.s.frame == B2_FRAME_ROWS || f.s.frame == B2_FRAME_RANGE || f.s.frame == B2_FRAME_RANGE_VALUE, "window: unknown frame type");
       B2_CHECK(f.s.lower != B2_UNBOUNDED_FOLLOWING && f.s.upper != B2_UNBOUNDED_PRECEDING, "window: frame bounds in the wrong direction");
       B2_CHECK(lu || uu || f.s.lower <= f.s.upper, "window: frame lower bound above the upper bound");
       if (f.s.frame == B2_FRAME_RANGE && !(lu && (uu || f.s.upper == 0)))
         throw Error(B2_ERR_UNSUPPORTED, "window: RANGE frames with value offsets");
+      if (f.s.frame == B2_FRAME_RANGE_VALUE) {
+        B2_CHECK(norder > 0 || (lu && uu), "window: a RANGE frame bounded by value needs ORDER BY");
+        B2_CHECK(norder == 1 || !(value_offset(f.s.lower) || value_offset(f.s.upper)), "window: RANGE value offsets need exactly one ORDER BY column");
+      }
+      // RANGE_VALUE (UNBOUNDED, 0) and (UNBOUNDED, UNBOUNDED) are RANGE's running and whole-partition frames
       if (lu && f.s.upper == 0) f.frame = f.s.frame == B2_FRAME_ROWS ? FR_ROWS_RUNNING : FR_RANGE_RUNNING;
+      else if (f.s.frame == B2_FRAME_RANGE_VALUE && !(lu && uu)) f.frame = FR_RANGE_VALUE;
       else f.frame = FR_GENERAL;
     } else {
       throw Error(B2_ERR_INVALID, "window: unknown function kind " + std::to_string(kind));
     }
-    const int m = (f.frame == FR_GENERAL) ? 3 : f.frame == FR_RANGE_RUNNING ? 2 : 1;
+    const int m = (f.frame == FR_GENERAL || f.frame == FR_RANGE_VALUE) ? 3 : f.frame == FR_RANGE_RUNNING ? 2 : 1;
     p.mode = std::max(p.mode, m);
     if (kind == B2_WIN_LAG) p.pre = std::max(p.pre, (int64_t)f.s.offset);
     else if (kind == B2_WIN_LEAD) p.post = std::max(p.post, (int64_t)f.s.offset);
@@ -525,6 +703,12 @@ void bind_window(WindowPlan& p, const Table* t) {
   for (auto& o : p.order) B2_CHECK(o.column >= 0 && o.column < nc, "window: order key column out of range");
   for (WinFn& f : p.fns) {
     const int kind = f.s.kind;
+    if (f.frame == FR_RANGE_VALUE && (value_offset(f.s.lower) || value_offset(f.s.upper))) {
+      const int ot = t->cols[p.order[0].column]->dtype;
+      if (is_float(ot)) throw Error(B2_ERR_UNSUPPORTED, "window: RANGE value offsets over a FLOAT ORDER BY column");
+      B2_CHECK(ot == B2_INT8 || ot == B2_INT16 || ot == B2_INT32 || ot == B2_INT64 || ot == B2_DATE32 || ot == B2_TIMESTAMP_US || is_decimal(ot),
+               "window: RANGE value offsets need an integer, DATE32, TIMESTAMP_US or decimal ORDER BY column");
+    }
     if (!needs_column(kind)) continue;
     B2_CHECK(f.s.column >= 0 && f.s.column < nc, "window: function column out of range");
     const int dt = t->cols[f.s.column]->dtype;
@@ -568,6 +752,31 @@ static void run_finish(const Op& op, const FrameArgs& fr, const Groups& g, const
   if (!rows) launch("window_finish_kernel", window_finish_kernel<Op, AllRows>, grid_for(n, 256), 256, 0, stream(), op, fr, g, state.as<T>(), AllRows{n}, o);
   else launch("window_finish_kernel", window_finish_kernel<Op, RowRange>, grid_for(rows->hi - rows->lo, 256), 256, 0, stream(), op, fr, g, state.as<T>(),
               RowRange{rows->lo, rows->hi}, o);
+}
+
+// a RANGE_VALUE function over every row of a chunk, from its frames se = [s[0..n), e[0..n)]
+template <class Op>
+static void run_range_finish(const Op& op, const Groups& g, const DevBuf& se, const DevBuf& state, int64_t n, const WinOut& o) {
+  using T = typename Op::T;
+  RangeTable<T> rt{nullptr, nullptr, nullptr, 0, 0};
+  DevBuf pre, suf, levels;
+  if constexpr (!Op::SUB) {
+    // 2 n + ~n / 512 states: 32 B per row for a 16-byte state
+    const int64_t ntiles = (n + WIN_TILE - 1) / WIN_TILE;
+    int nlev = 1;
+    while (((int64_t)1 << nlev) <= ntiles) nlev++;
+    pre = DevBuf((size_t)n * sizeof(T));
+    suf = DevBuf((size_t)n * sizeof(T));
+    levels = DevBuf((size_t)nlev * ntiles * sizeof(T));
+    T* lv = levels.as<T>();
+    launch("window_range_tiles_kernel", window_range_tiles_kernel<Op>, grid_for(ntiles, 1, 8), WIN_NT, 0, stream(), op, n, pre.as<T>(), suf.as<T>(), lv);
+    for (int k = 1; k < nlev; k++)
+      launch("window_range_table_kernel", window_range_table_kernel<Op>, grid_for(ntiles, 256), 256, 0, stream(), op, ntiles, (int64_t)1 << (k - 1),
+             (const T*)(lv + (int64_t)(k - 1) * ntiles), lv + (int64_t)k * ntiles);
+    rt = RangeTable<T>{pre.as<T>(), suf.as<T>(), lv, ntiles, nlev};
+  }
+  const int32_t* s = se.as<int32_t>();
+  launch("window_range_finish_kernel", window_range_finish_kernel<Op>, grid_for(n, 256), 256, 0, stream(), op, g, s, s + n, state.as<T>(), rt, n, o);
 }
 
 static SortPlan empty_plan() { SortPlan p; memset(&p, 0, sizeof(p)); return p; }
@@ -639,7 +848,10 @@ static std::vector<Column*> window_functions(WindowPlan& p, const Table* t, Wind
   DevBuf rank = n ? run_scan(rop, fl, n, has_state ? &carry->state[0] : nullptr, next_state[0]) : DevBuf();
   if (rows && carry_row >= 0) carry_at<RankOp::T>(rank, carry_row, next_state[0]);
   bool need_pend = false, need_peer = false;
-  for (const WinFn& f : p.fns) { need_pend = need_pend || f.frame == FR_GENERAL; need_peer = need_peer || f.frame == FR_RANGE_RUNNING; }
+  for (const WinFn& f : p.fns) {
+    need_pend = need_pend || f.frame == FR_GENERAL || f.frame == FR_RANGE_VALUE;
+    need_peer = need_peer || f.frame == FR_RANGE_RUNNING || f.frame == FR_RANGE_VALUE;
+  }
   DevBuf pend, peer;
   if (n && (need_pend || need_peer)) {
     if (need_pend) pend = DevBuf((size_t)n * 4);
@@ -648,6 +860,26 @@ static std::vector<Column*> window_functions(WindowPlan& p, const Table* t, Wind
            peer.as<int32_t>());
   }
   const Groups g{rank.as<RankOp::T>(), pend.as<int32_t>(), peer.as<int32_t>()};
+
+  // the frames of each distinct RANGE_VALUE (lower, upper), computed once and shared by the functions that use it
+  std::vector<std::pair<std::pair<int64_t, int64_t>, DevBuf>> range_frames;
+  auto frames_of = [&](const WinFn& f) -> const DevBuf& {
+    const std::pair<int64_t, int64_t> key{f.s.lower, f.s.upper};
+    for (auto& rf : range_frames)
+      if (rf.first == key) return rf.second;
+    B2_CHECK(!rows, "window: RANGE frames with value offsets do not stream");
+    RangeKey rk{ColView{}, 0, 0};
+    if (value_offset(f.s.lower) || value_offset(f.s.upper)) {
+      rk.col = view_of(t->cols[p.order[0].column]);
+      rk.desc = p.order[0].ascending ? 0 : 1;
+      rk.nulls_first = p.order[0].nulls_first ? 1 : 0;
+    }
+    const RangeBounds b{f.s.lower, f.s.upper, f.s.lower == B2_UNBOUNDED_PRECEDING, f.s.upper == B2_UNBOUNDED_FOLLOWING};
+    DevBuf se((size_t)n * 8);
+    launch("window_range_bounds_kernel", window_range_bounds_kernel, grid_for(n, 256), 256, 0, stream(), rk, b, g, n, se.as<int32_t>(), se.as<int32_t>() + n);
+    range_frames.emplace_back(key, std::move(se));
+    return range_frames.back().second;
+  };
 
   ColsGuard outs;
   for (size_t k = 0; k < nf; k++) {
@@ -694,7 +926,8 @@ static std::vector<Column*> window_functions(WindowPlan& p, const Table* t, Wind
       using T = typename std::decay_t<decltype(op)>::T;
       DevBuf st = run_scan(op, fl, n, cin, next_state[k + 1]);
       if (rows && carry_row >= 0) carry_at<T>(st, carry_row, next_state[k + 1]);
-      run_finish(op, fr, g, st, n, o, rows);
+      if (f.frame == FR_RANGE_VALUE) run_range_finish(op, g, frames_of(f), st, n, o);
+      else run_finish(op, fr, g, st, n, o, rows);
     };
     if (is_ranking(kind)) run_finish(rop, fr, g, rank, n, o, rows);
     else if (kind == B2_WIN_COUNT || kind == B2_WIN_COUNT_ALL) scan_finish(CountOp{in ? view_of(in) : ColView{}, kind == B2_WIN_COUNT_ALL});

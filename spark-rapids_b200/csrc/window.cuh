@@ -14,7 +14,7 @@ struct WindowPlan {
   std::vector<int32_t> part;
   std::vector<b2_order_by_arg> order;
   std::vector<WinFn> fns;
-  int mode = 1;   // 1 running only, 2 a RANGE running frame, 3 a frame that needs the whole partition (or LEAD / LAG)
+  int mode = 1;   // 1 running only, 2 a RANGE running frame, 3 a frame that needs the whole partition (LEAD / LAG, RANGE value offsets)
   // P and F: how many rows before (pre) and after (post) a row its frame or LEAD / LAG source can reach.  bounded: every function
   // is ranking, LEAD / LAG or a ROWS frame with a finite upper bound, and P + F > 0; such a plan streams with context rows
   int64_t pre = 0, post = 0;
