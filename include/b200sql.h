@@ -380,7 +380,10 @@ int b2_concat(const b2_handle* tables, int32_t ntables, b2_handle* out_table);
 int b2_serialized_size(b2_handle table, int64_t row_start, int64_t row_end, int64_t* out_bytes);
 int b2_serialize_table(b2_handle table, int64_t row_start, int64_t row_end, uint8_t* host_out, int64_t capacity,
                        int64_t* out_written);
-/* N serialised tables -> one device table: concatenated on the host, one upload per column buffer */
+/* N serialised tables -> one device table: concatenated on the host, one upload per column buffer.  B2_ERR_INVALID when a
+ * buffer is not self-consistent: a descriptor whose sizes disagree with the row count or null_count, buffers past
+ * total_bytes, string offsets that do not run from 0 to data_bytes without decreasing, or inputs that differ in column
+ * count, type or scale.  Validity bits past an input's last row are ignored. */
 int b2_deserialize_concat(const uint8_t* const* bufs, const int64_t* lens, int32_t nbufs, b2_handle* out_table);
 
 /* ---- (e) exchange: RapidsShuffleManager replaced by NCCL all-to-all over NVLink ---------------

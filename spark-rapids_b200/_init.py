@@ -843,6 +843,16 @@ class Comm:
                                    ctypes.byref(out), ctypes.byref(anyd)))
         return (Table(out.value) if out.value else None), bool(anyd.value)
 
+    def exchange_hash_sel(self, table, key_cols, selection=None, out_cols=None, seed=42):
+        """exchange_hash over the rows of `table` that the INT32 column `selection` names (all rows when None), sending only
+        the columns `out_cols` (all when None); key_cols index `table` itself.  -> (Table|None, any_data)"""
+        out, anyd = ctypes.c_int64(), ctypes.c_int32()
+        oc = None if not out_cols else _i32s(out_cols)
+        check(lib.b2_exchange_hash_sel(self.h, table.h if table is not None else ctypes.c_int64(0),
+                                       selection.h if selection is not None else ctypes.c_int64(0), oc, len(out_cols or []),
+                                       _i32s(key_cols), len(key_cols), seed, ctypes.byref(out), ctypes.byref(anyd)))
+        return (Table(out.value) if out.value else None), bool(anyd.value)
+
     def fused_ready(self):
         ok = ctypes.c_int32()
         check(lib.b2_comm_fused_ready(self.h, ctypes.byref(ok)))

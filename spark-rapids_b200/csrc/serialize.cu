@@ -11,8 +11,8 @@
 //
 //   SerHeader { u32 magic 'B2T1'; u16 version = 1; u16 ncols; i64 rows; i64 total_bytes }              24 bytes
 //   SerCol[ncols] { i32 dtype; i32 scale; i64 null_count; i64 validity_bytes; i64 offsets_bytes; i64 data_bytes }   40 bytes each
-//   padding to 64, then for every column: validity (LSB-first bits, absent when null_count == 0) | offsets (int32,
-//   rebased to 0, STRING only) | data — each padded to a multiple of 64 bytes.
+//   padding to 64, then for every column: validity (LSB-first bits, absent when null_count == 0; the reader ignores the
+//   bits past the last row) | offsets (int32, rebased to 0, STRING only) | data — each padded to a multiple of 64 bytes.
 #include <algorithm>
 #include <deque>
 #include "common.cuh"
@@ -102,6 +102,33 @@ int b2_serialize_table(b2_handle table, int64_t row_start, int64_t row_end, uint
   B2_CATCH
 }
 
+// A descriptor must agree with its table's row count, and its buffers must lie inside the serialised table: the reader
+// copies by row count, so a descriptor that declares fewer bytes than its rows need would make it read past the buffer.
+// String offsets must start at 0, never decrease and end at data_bytes; set bits must number rows - null_count.
+static void check_column(const uint8_t* buf, const SerHeader& h, const SerCol& sc, int64_t cur) {
+  const int64_t n = h.rows;
+  const bool str = sc.dtype == B2_STRING;
+  B2_CHECK(sc.dtype >= B2_BOOL8 && sc.dtype <= B2_STRING, "serialised column has an unknown type");
+  B2_CHECK(sc.null_count >= 0 && sc.null_count <= n, "serialised column: null_count out of range");
+  B2_CHECK(sc.validity_bytes == (sc.null_count > 0 ? (n + 7) / 8 : 0), "serialised column: validity_bytes disagrees with rows / null_count");
+  B2_CHECK(sc.offsets_bytes == (str ? (n + 1) * 4 : 0), "serialised column: offsets_bytes disagrees with rows");
+  B2_CHECK(str ? sc.data_bytes >= 0 : sc.data_bytes == n * dtype_width(sc.dtype), "serialised column: data_bytes disagrees with rows");
+  B2_CHECK(sc.data_bytes <= h.total_bytes && cur + pad64i(sc.validity_bytes) + pad64i(sc.offsets_bytes) + pad64i(sc.data_bytes) <= h.total_bytes,
+           "serialised table is truncated");
+  if (sc.validity_bytes) {
+    const uint8_t* v = buf + cur;
+    int64_t set = 0;
+    for (int64_t k = 0; k < n / 8; k++) set += __builtin_popcount(v[k]);
+    if (n & 7) set += __builtin_popcount(v[n / 8] & ((1u << (n & 7)) - 1u));
+    B2_CHECK(set == n - sc.null_count, "serialised column: null_count disagrees with the validity bits");
+  }
+  if (str) {
+    const int32_t* o = reinterpret_cast<const int32_t*>(buf + cur + pad64i(sc.validity_bytes));
+    B2_CHECK(o[0] == 0 && o[n] == sc.data_bytes, "serialised string offsets must run from 0 to data_bytes");
+    for (int64_t r = 0; r < n; r++) B2_CHECK(o[r] <= o[r + 1], "serialised string offsets decrease");
+  }
+}
+
 // GpuShuffleCoalesceExec: N serialised tables -> ONE device table; the concatenation happens on the host (validity bits
 // shifted into place, string offsets rebased), then each column buffer is uploaded once.
 int b2_deserialize_concat(const uint8_t* const* bufs, const int64_t* lens, int32_t nbufs, b2_handle* out_table) {
@@ -114,8 +141,9 @@ int b2_deserialize_concat(const uint8_t* const* bufs, const int64_t* lens, int32
     B2_CHECK(lens[b] >= (int64_t)sizeof(SerHeader), "serialised table is truncated");
     const SerHeader* h = reinterpret_cast<const SerHeader*>(bufs[b]);
     B2_CHECK(h->magic == SER_MAGIC && h->version == 1, "not a B2T1 serialised table");
-    B2_CHECK(h->total_bytes <= lens[b] && h->rows >= 0, "serialised table is truncated");
     B2_CHECK(h->ncols == reinterpret_cast<const SerHeader*>(bufs[0])->ncols, "serialised tables differ in column count");
+    B2_CHECK(h->total_bytes <= lens[b] && h->total_bytes >= pad64i((int64_t)sizeof(SerHeader) + (int64_t)h->ncols * (int64_t)sizeof(SerCol)) &&
+             h->rows >= 0 && h->rows <= 0x7fffffffLL, "serialised table is truncated");
     hs.push_back(h);
     cs.push_back(reinterpret_cast<const SerCol*>(bufs[b] + sizeof(SerHeader)));
     rows += h->rows;
@@ -132,7 +160,8 @@ int b2_deserialize_concat(const uint8_t* const* bufs, const int64_t* lens, int32
     const int dtype = cs[0][i].dtype;
     int64_t nulls = 0, chars = 0;
     for (int b = 0; b < nbufs; b++) {
-      B2_CHECK(cs[b][i].dtype == dtype, "serialised tables differ in column type");
+      B2_CHECK(cs[b][i].dtype == dtype && cs[b][i].scale == cs[0][i].scale, "serialised tables differ in column type");
+      check_column(bufs[b], *hs[b], cs[b][i], cur[b]);
       nulls += cs[b][i].null_count; chars += cs[b][i].data_bytes;
     }
     if (dtype == B2_STRING && chars > 0x7fffffffLL) throw Error(B2_ERR_SIZE_OVERFLOW, "coalesced string column exceeds 2^31-1 chars");
@@ -152,10 +181,14 @@ int b2_deserialize_concat(const uint8_t* const* bufs, const int64_t* lens, int32
       const uint8_t* v = bufs[b] + cur[b]; cur[b] += pad64i(sc.validity_bytes);
       const uint8_t* o = bufs[b] + cur[b]; cur[b] += pad64i(sc.offsets_bytes);
       const uint8_t* d = bufs[b] + cur[b]; cur[b] += pad64i(sc.data_bytes);
-      B2_CHECK(cur[b] <= hs[b]->total_bytes, "serialised table is truncated");
       if (nulls > 0) {
         if (sc.validity_bytes == 0) { for (int64_t r = 0; r < n; r++) vbuf[(size_t)((row + r) >> 3)] |= (uint8_t)(1u << ((row + r) & 7)); }
-        else if ((row & 7) == 0) memcpy(vbuf.data() + (row >> 3), v, (size_t)((n + 7) / 8));
+        else if ((row & 7) == 0) {
+          uint8_t* dst = vbuf.data() + (row >> 3);
+          memcpy(dst, v, (size_t)((n + 7) / 8));
+          // the writer need not zero the bits past its last row: they would mark the next input's first rows valid
+          if (n & 7) dst[n >> 3] &= (uint8_t)((1u << (n & 7)) - 1u);
+        }
         else for (int64_t r = 0; r < n; r++) if ((v[r >> 3] >> (r & 7)) & 1) vbuf[(size_t)((row + r) >> 3)] |= (uint8_t)(1u << ((row + r) & 7));
       }
       if (dtype == B2_STRING) {
@@ -167,7 +200,6 @@ int b2_deserialize_concat(const uint8_t* const* bufs, const int64_t* lens, int32
       } else if (n) memcpy(dbuf.data() + row * w, d, (size_t)(n * w));
       row += n;
     }
-    if (nulls > 0 && (rows & 7)) vbuf[(size_t)(rows >> 3)] &= (uint8_t)((1u << (rows & 7)) - 1u);
     if (dtype == B2_STRING) {
       reinterpret_cast<int32_t*>(obuf.data())[rows] = (int32_t)ch;
       oc->offsets = DevBuf(obuf.size());
