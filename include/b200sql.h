@@ -450,10 +450,20 @@ int b2_broadcast_table(b2_handle comm, b2_handle table, int32_t root, b2_handle*
  *   MAX a range query whose work per row does not grow with the frame (32 B per row of device memory per such function for
  *   its 16-byte state).  Bounds of only 0 and UNBOUNDED need peer groups only and take any ORDER BY.  Errors, B2_ERR_INVALID:
  *   no ORDER BY with a bound other than UNBOUNDED; lower > upper or a bound in the wrong direction; a value offset with more
- *   than one ORDER BY column or over a STRING or BOOL8 one.  B2_ERR_UNSUPPORTED: a value offset over FLOAT32 / FLOAT64. */
+ *   than one ORDER BY column or over a STRING or BOOL8 one.  B2_ERR_UNSUPPORTED: a value offset over FLOAT32 / FLOAT64.
+ * FIRST / LAST / NTH_VALUE (GpuFirst / GpuLast / GpuNthValue, aggregateFunctions.scala; FirstRunningWindowFixer and
+ *   LastRunningWindowFixer, GpuWindowExpression.scala) -> the column's type and scale, any type (BOOL8, STRING, DECIMAL128
+ *   included), the value copied bit for bit (NaN payloads, -0.0, "" apart from NULL).  Frames, their errors and their batching
+ *   are exactly SUM's.  For the frame [s, e] of a row: FIRST is the value at s, LAST the value at e, NTH_VALUE the value at
+ *   s + n - 1 with n in `offset` (n < 1: B2_ERR_INVALID); NULL when the frame is empty or holds fewer than n rows.  With
+ *   ignore_nulls, rows whose value is NULL do not count: the first, last or n-th non-NULL value of the frame, NULL when there is
+ *   none.  Each row's source row is found without a loop over its frame (a select on a rank directory of the validity words,
+ *   1/8 byte per row, for IGNORE NULLS over a column with NULLs), and the values are gathered as LEAD / LAG's.  ignore_nulls on
+ *   LEAD / LAG: B2_ERR_UNSUPPORTED; on any other kind: B2_ERR_INVALID. */
 typedef enum {
   B2_WIN_ROW_NUMBER = 1, B2_WIN_RANK = 2, B2_WIN_DENSE_RANK = 3, B2_WIN_LEAD = 4, B2_WIN_LAG = 5,
-  B2_WIN_SUM = 10, B2_WIN_COUNT = 11, B2_WIN_COUNT_ALL = 12, B2_WIN_MIN = 13, B2_WIN_MAX = 14
+  B2_WIN_SUM = 10, B2_WIN_COUNT = 11, B2_WIN_COUNT_ALL = 12, B2_WIN_MIN = 13, B2_WIN_MAX = 14,
+  B2_WIN_FIRST = 15, B2_WIN_LAST = 16, B2_WIN_NTH_VALUE = 17
 } b2_window_kind;
 typedef enum { B2_FRAME_ROWS = 0, B2_FRAME_RANGE = 1, B2_FRAME_RANGE_VALUE = 2 } b2_frame_type;
 #define B2_UNBOUNDED_PRECEDING INT64_MIN
@@ -461,11 +471,12 @@ typedef enum { B2_FRAME_ROWS = 0, B2_FRAME_RANGE = 1, B2_FRAME_RANGE_VALUE = 2 }
 typedef struct {
   int32_t kind, column;            /* column ignored by ROW_NUMBER / RANK / DENSE_RANK / COUNT_ALL */
   int32_t frame;                   /* b2_frame_type; ignored by the ranking functions and LEAD / LAG */
-  int32_t offset;                  /* LEAD / LAG, >= 0 */
+  int32_t offset;                  /* LEAD / LAG, >= 0; NTH_VALUE's n, >= 1 */
   int64_t lower, upper;            /* frame bounds */
   uint8_t default_value[16];       /* LEAD / LAG default, b2_expr_literal's encoding */
   int32_t default_is_null;
   int32_t out_dtype, out_precision, out_scale;   /* read by decimal SUM only (DECIMAL64 or DECIMAL128; scale = the input's) */
+  int32_t ignore_nulls;            /* FIRST / LAST / NTH_VALUE: IGNORE NULLS; 0 = RESPECT NULLS */
 } b2_window_spec;
 /* one sorted batch: output = the input columns, then one column per spec */
 int b2_window(b2_handle table, const int32_t* part_cols, int32_t nparts, const b2_order_by_arg* order, int32_t norder,

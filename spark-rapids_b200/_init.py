@@ -27,6 +27,7 @@ AGG_SUM, AGG_COUNT, AGG_MIN, AGG_MAX, AGG_COUNT_ALL = 1, 2, 3, 4, 5
 # b2_window_kind, b2_frame_type
 WIN_ROW_NUMBER, WIN_RANK, WIN_DENSE_RANK, WIN_LEAD, WIN_LAG = 1, 2, 3, 4, 5
 WIN_SUM, WIN_COUNT, WIN_COUNT_ALL, WIN_MIN, WIN_MAX = 10, 11, 12, 13, 14
+WIN_FIRST, WIN_LAST, WIN_NTH_VALUE = 15, 16, 17
 FRAME_ROWS, FRAME_RANGE, FRAME_RANGE_VALUE = 0, 1, 2
 UNBOUNDED_PRECEDING, UNBOUNDED_FOLLOWING = -2**63, 2**63 - 1
 # b2_join_kind
@@ -446,13 +447,16 @@ def unbounded():
 
 
 class WindowFunc:
-    """one window function: kind (WIN_*), its column, a Frame (aggregates), LEAD / LAG offset and default, and for a decimal
-    SUM the result type (out_dtype, out_precision; the scale is the input's)"""
+    """one window function: kind (WIN_*), its column, a Frame (aggregates, FIRST / LAST / NTH_VALUE), LEAD / LAG offset and
+    default or NTH_VALUE's n (in offset), for a decimal SUM the result type (out_dtype, out_precision; the scale is the input's),
+    and IGNORE NULLS for FIRST / LAST / NTH_VALUE"""
 
-    def __init__(self, kind, column=0, frame=None, offset=1, default=None, default_dtype=None, out_dtype=0, out_precision=0):
+    def __init__(self, kind, column=0, frame=None, offset=1, default=None, default_dtype=None, out_dtype=0, out_precision=0,
+                 ignore_nulls=False):
         self.kind, self.column, self.frame, self.offset = kind, column, frame, offset
         self.default, self.default_dtype = default, default_dtype
         self.out_dtype, self.out_precision = out_dtype, out_precision
+        self.ignore_nulls = ignore_nulls
 
 
 def row_number():
@@ -503,6 +507,21 @@ def win_max(column, frame):
     return WindowFunc(WIN_MAX, column, frame)
 
 
+def first_value(column, frame, ignore_nulls=False):
+    """first_value(column) [IGNORE NULLS] over frame: the value at the frame's first row (the first non-NULL one)"""
+    return WindowFunc(WIN_FIRST, column, frame, ignore_nulls=ignore_nulls)
+
+
+def last_value(column, frame, ignore_nulls=False):
+    """last_value(column) [IGNORE NULLS] over frame; with rows(None, 0) and ignore_nulls, a forward fill"""
+    return WindowFunc(WIN_LAST, column, frame, ignore_nulls=ignore_nulls)
+
+
+def nth_value(column, n, frame, ignore_nulls=False):
+    """nth_value(column, n) [IGNORE NULLS] over frame: the value at the frame's n-th row (n-th non-NULL one), n >= 1"""
+    return WindowFunc(WIN_NTH_VALUE, column, frame, offset=n, ignore_nulls=ignore_nulls)
+
+
 def _literal16(value, dtype):
     buf = np.zeros(2, dtype=np.uint64)
     if dtype == FLOAT32:
@@ -532,6 +551,7 @@ def _window_specs(funcs):
         if f.default is not None:
             s.default_value[:] = list(_literal16(f.default, f.default_dtype))
         s.out_dtype, s.out_precision = f.out_dtype, f.out_precision
+        s.ignore_nulls = int(bool(f.ignore_nulls))
     return arr
 
 

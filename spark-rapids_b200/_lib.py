@@ -39,7 +39,7 @@ class B2WindowSpec(ctypes.Structure):
     _fields_ = [("kind", ctypes.c_int32), ("column", ctypes.c_int32), ("frame", ctypes.c_int32), ("offset", ctypes.c_int32),
                 ("lower", ctypes.c_int64), ("upper", ctypes.c_int64), ("default_value", ctypes.c_uint8 * 16),
                 ("default_is_null", ctypes.c_int32), ("out_dtype", ctypes.c_int32), ("out_precision", ctypes.c_int32),
-                ("out_scale", ctypes.c_int32)]
+                ("out_scale", ctypes.c_int32), ("ignore_nulls", ctypes.c_int32)]
 
 
 def _arg_type(decl):

@@ -16,7 +16,11 @@
 //                             at the partition's end), a difference of prefixes for integer, decimal and count sums, otherwise a
 //                             loop over the frame (float SUM, MIN, MAX: O(rows x frame width), as cudf's rolling window)
 //   window_lead_lag_kernel    LEAD / LAG source row (or -1 outside the partition); values through gather_table, then the default
-// Finish and LEAD / LAG run over every row of the chunk (AllRows) or, for a streamed bounded plan, only over the rows [lo, hi)
+//   window_value_kernel       FIRST / LAST / NTH_VALUE source row of each row's frame (or -1: NULL, or n: the carried value), with
+//                             IGNORE NULLS a select on a rank directory of the validity words (window_valid_popc_kernel + a
+//                             scan); values through gather_table, then window_value_patch_kernel writes the carried value.
+//                             window_value_carry_kernel takes the next carry (count and source row) at the carry row
+// Finish, LEAD / LAG and the value functions run over every row of the chunk (AllRows) or, for a streamed bounded plan, only over the rows [lo, hi)
 // between its context and look-ahead rows (RowRange), writing columns of hi - lo rows.
 // RANGE frames with value offsets (B2_FRAME_RANGE_VALUE; BasicWindowCalc.scala:169-219, 445 aggregateWindowsOverRanges):
 //   window_range_bounds_kernel  each row's frame [s, e], once per distinct (lower, upper): a binary search of the ORDER BY
@@ -28,6 +32,7 @@
 //                               otherwise suffix[s] + O(log tiles) levels + prefix[e] (a loop when s and e share a tile), so
 //                               the work per row is bounded by WIN_TILE + log2(tiles) whatever the frame's width
 #include <algorithm>
+#include "prim.cuh"
 #include "sortkey.cuh"
 #include "window.cuh"
 
@@ -450,6 +455,127 @@ __global__ void window_default_kernel(const int32_t* __restrict__ map, int64_t n
 }
 
 // ------------------------------------------------------------------------------------------------
+// FIRST / LAST / NTH_VALUE (GpuFirst / GpuLast / GpuNthValue: RollingAggregation.nth with a NullPolicy): each row's source row
+// in a map, the values then gathered through it
+
+// dir[w] = the valid rows of validity words [0, w): per-word popcounts here (padding bits past row n - 1 masked), then an
+// exclusive scan that also writes dir[nwords]
+__global__ void window_valid_popc_kernel(const uint32_t* __restrict__ valid, int64_t n, int64_t nwords, int32_t* __restrict__ cnt) {
+  for (int64_t w = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; w < nwords; w += (int64_t)gridDim.x * blockDim.x) {
+    const int tail = (int)(n - w * 32);
+    cnt[w] = __popc(tail >= 32 ? valid[w] : valid[w] & ((1u << tail) - 1));
+  }
+}
+
+struct ValueFn {
+  int32_t last;            // LAST; otherwise FIRST (nth = 1) or NTH_VALUE
+  int64_t nth;
+  const uint32_t* valid;   // with dir: the column's validity words
+  const int32_t* dir;      // IGNORE NULLS over a column with NULLs: the rank directory; null: every row counts
+  int64_t n;               // the chunk's rows, also the source row that stands for the carried value
+  const int64_t* c0;       // the carried count: the open partition's counted rows before row 0, or null
+
+  // counted rows in [0, x), 0 <= x <= n
+  __device__ __forceinline__ int64_t before(int64_t x) const {
+    const int64_t w = x >> 5;
+    const int b = (int)(x & 31);
+    return dir[w] + (b ? __popc(valid[w] & ((1u << b) - 1)) : 0);
+  }
+  // the row of the counted row of rank t (0-based, t < the chunk's count): the word w with dir[w] <= t < dir[w + 1], galloped for
+  // from word `from` in whichever direction holds it and then bisected, so the work grows with the log of the distance; then the
+  // (t - dir[w] + 1)-th set bit of the word
+  __device__ int64_t select(int64_t t, int64_t from) const {
+    const int64_t nw = (n + 31) >> 5;
+    int64_t lo, hi;   // dir[lo] <= t < dir[hi]
+    if (dir[from] <= t) {
+      lo = from;
+      for (int64_t d = 1;; d <<= 1) {
+        hi = min(from + d, nw);
+        if (dir[hi] > t) break;
+        lo = hi;
+      }
+    } else {
+      hi = from;
+      for (int64_t d = 1;; d <<= 1) {
+        lo = max(from - d, (int64_t)0);
+        if (dir[lo] <= t) break;
+        hi = lo;
+      }
+    }
+    while (hi - lo > 1) {
+      const int64_t mid = lo + ((hi - lo) >> 1);
+      if (dir[mid] <= t) lo = mid;
+      else hi = mid;
+    }
+    return lo * 32 + __fns(valid[lo], 0, (int)(t - dir[lo]) + 1);
+  }
+  // The source row of the frame [s, e] (s <= e unless cont), -1 for NULL, n for the carried value.  cont: the frame starts
+  // where the partition does, before row 0 (s = 0); then c0 rows came before it.  e >= 0 there, as a continuing frame always
+  // reaches row 0 (running frames; a bounded chunk's output rows have i + upper >= 1).
+  __device__ int64_t src(int64_t s, int64_t e, bool cont) const {
+    const int64_t c = cont && c0 ? *c0 : 0;
+    if (last) {
+      if (!dir) return e;
+      const int64_t k = before(e + 1);
+      if (k > before(s)) return select(k - 1, e >> 5);
+      return c > 0 ? n : -1;
+    }
+    if (c >= nth) return n;
+    const int64_t k = nth - c;   // the k-th counted row from s
+    if (!dir) return s + k - 1 <= e ? s + k - 1 : -1;
+    const int64_t t = before(s) + k - 1;
+    return t < before(e + 1) ? select(t, s >> 5) : -1;
+  }
+};
+
+// map[out(i)] = the source row of row i's frame, found as window_finish_kernel finds [s, e] (RANGE_VALUE: s_at, e_at)
+template <class R>
+__global__ void window_value_kernel(const ValueFn f, const FrameArgs fr, const Groups g, const int32_t* __restrict__ s_at,
+                                    const int32_t* __restrict__ e_at, const R rows, int32_t* __restrict__ map) {
+  for (int64_t i = rows.begin() + blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < rows.end(); i += (int64_t)gridDim.x * blockDim.x) {
+    const RankOp::T r = g.rank[i];
+    const int64_t p = i - r.rn + 1, ps = max((int64_t)0, p);
+    int64_t s = ps, e = i;
+    bool from_ps = true;
+    if (fr.type == FR_RANGE_RUNNING) {
+      e = g.peer_end_at[max((int64_t)0, i - r.rn + r.rk)];
+    } else if (fr.type == FR_GENERAL) {
+      const int64_t pe = g.pend_at[ps];
+      s = fr.lower_unb ? ps : max(ps, i + fr.lower);
+      e = fr.upper_unb ? pe : min(pe, i + fr.upper);
+      from_ps = fr.lower_unb;
+    } else if (fr.type == FR_RANGE_VALUE) {
+      s = s_at[i];
+      e = e_at[i];
+      from_ps = false;
+    }
+    const bool cont = from_ps && p < 0;
+    map[rows.out(i)] = (!cont && s > e) ? -1 : (int32_t)f.src(s, e, cont);
+  }
+}
+
+// the carry at row r (one thread): the count of the open partition's counted rows up to r, and the source row of the value its
+// continuing frames resolve to (the frame [partition start, r])
+__global__ void window_value_carry_kernel(const ValueFn f, const RankOp::T* __restrict__ rank, int64_t r, int64_t* __restrict__ count,
+                                          int32_t* __restrict__ map) {
+  const int64_t p = r - rank[r].rn + 1, s = max((int64_t)0, p);
+  const bool cont = p < 0;
+  *count = (cont && f.c0 ? *f.c0 : 0) + (f.dir ? f.before(r + 1) - f.before(s) : r - s + 1);
+  *map = (int32_t)f.src(s, r, cont);
+}
+
+// the rows whose source is the carried value (map[i] == mark; the gather left them NULL) take its bytes and validity
+__global__ void window_value_patch_kernel(const int32_t* __restrict__ map, int64_t m, int32_t mark, const void* __restrict__ cdata,
+                                          const uint32_t* __restrict__ cvalid, int width, void* __restrict__ data, uint32_t* __restrict__ valid) {
+  if (!row_valid(cvalid, 0)) return;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < m; i += (int64_t)gridDim.x * blockDim.x) {
+    if (map[i] != mark) continue;
+    memcpy(reinterpret_cast<char*>(data) + i * width, cdata, width);
+    atomicOr(&valid[i >> 5], 1u << (i & 31));
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
 // RANGE frames with value offsets (Spark's RangeBoundOrdering)
 
 // The first ORDER BY column as a key that ascends in the sort order: x, or -x for DESC, exact in 128 bits, so that the bound
@@ -614,6 +740,7 @@ __global__ void window_range_finish_kernel(const Op op, const Groups g, const in
 // host side
 static bool is_ranking(int k) { return k == B2_WIN_ROW_NUMBER || k == B2_WIN_RANK || k == B2_WIN_DENSE_RANK; }
 static bool is_offset_fn(int k) { return k == B2_WIN_LEAD || k == B2_WIN_LAG; }
+static bool is_value_fn(int k) { return k == B2_WIN_FIRST || k == B2_WIN_LAST || k == B2_WIN_NTH_VALUE; }
 static bool needs_column(int k) { return !is_ranking(k) && k != B2_WIN_COUNT_ALL; }
 // a RANGE_VALUE bound that is a value offset (not CURRENT ROW, not UNBOUNDED)
 static bool value_offset(int64_t b) { return b != 0 && b != B2_UNBOUNDED_PRECEDING && b != B2_UNBOUNDED_FOLLOWING; }
@@ -634,6 +761,10 @@ WindowPlan make_window_plan(const int32_t* part_cols, int nparts, const b2_order
     WinFn f;
     f.s = specs[k];
     const int kind = f.s.kind;
+    if (f.s.ignore_nulls && !is_value_fn(kind)) {
+      if (is_offset_fn(kind)) throw Error(B2_ERR_UNSUPPORTED, "window: LEAD / LAG IGNORE NULLS");
+      throw Error(B2_ERR_INVALID, "window: IGNORE NULLS on a function other than FIRST / LAST / NTH_VALUE");
+    }
     if (is_ranking(kind) || is_offset_fn(kind)) {
       B2_CHECK(norder > 0, "window: ranking functions and LEAD / LAG need ORDER BY");
       f.frame = FR_ROWS_RUNNING;
@@ -641,7 +772,8 @@ WindowPlan make_window_plan(const int32_t* part_cols, int nparts, const b2_order
         B2_CHECK(f.s.offset >= 0, "window: LEAD / LAG offset must be >= 0");
         f.frame = FR_GENERAL;
       }
-    } else if (kind == B2_WIN_SUM || kind == B2_WIN_COUNT || kind == B2_WIN_COUNT_ALL || kind == B2_WIN_MIN || kind == B2_WIN_MAX) {
+    } else if (kind == B2_WIN_SUM || kind == B2_WIN_COUNT || kind == B2_WIN_COUNT_ALL || kind == B2_WIN_MIN || kind == B2_WIN_MAX || is_value_fn(kind)) {
+      B2_CHECK(kind != B2_WIN_NTH_VALUE || f.s.offset >= 1, "window: NTH_VALUE needs n >= 1");
       const bool lu = f.s.lower == B2_UNBOUNDED_PRECEDING, uu = f.s.upper == B2_UNBOUNDED_FOLLOWING;
       B2_CHECK(f.s.frame == B2_FRAME_ROWS || f.s.frame == B2_FRAME_RANGE || f.s.frame == B2_FRAME_RANGE_VALUE, "window: unknown frame type");
       B2_CHECK(f.s.lower != B2_UNBOUNDED_FOLLOWING && f.s.upper != B2_UNBOUNDED_PRECEDING, "window: frame bounds in the wrong direction");
@@ -829,6 +961,35 @@ static void carry_at(const DevBuf& state, int64_t r, DevBuf& carry) {
   CUDA_CHECK(cudaMemcpyAsync(carry.p, state.as<char>() + (size_t)r * sizeof(T), sizeof(T), cudaMemcpyDeviceToDevice, stream()));
 }
 
+// Column c of t gathered through map (m rows, out of range = NULL) as a value function's result; the rows whose source is t->rows
+// take cv, the one-row carried value
+static Column* gather_values(const Table* t, int c, const int32_t* map, int64_t m, const Column* cv) {
+  using TablePtr = std::unique_ptr<Table, void (*)(Table*)>;
+  const std::vector<int> only{c};
+  Column* oc;
+  if (cv && t->cols[c]->dtype == B2_STRING) {
+    // a STRING carried value is gathered from the column with it appended as row t->rows (a copy of the column's offsets and
+    // chars); a fixed-width column is never copied, its carried rows are patched below
+    Column *a = t->cols[c], *b = const_cast<Column*>(cv);
+    col_incref(a);
+    col_incref(b);
+    TablePtr ta(new_table({a}), table_release), tb(new_table({b}), table_release);
+    TablePtr both(concat_tables({ta.get(), tb.get()}), table_release);
+    TablePtr got(gather_table(both.get(), map, m, true, nullptr), table_release);
+    oc = got->cols[0];
+    col_incref(oc);
+  } else {
+    TablePtr got(gather_table(t, map, m, true, &only), table_release);
+    oc = got->cols[0];
+    col_incref(oc);
+    if (cv && m)
+      launch("window_value_patch_kernel", window_value_patch_kernel, grid_for(m, 256), 256, 0, stream(), map, m, (int32_t)t->rows, (const void*)cv->data.p,
+             cv->validity(), dtype_width(oc->dtype), oc->data.p, oc->valid.as<uint32_t>());
+  }
+  finalize_nulls(oc);
+  return oc;
+}
+
 // The functions over one chunk of rows sorted by (partition, order), one column per function.  With `rows`, only the rows
 // [lo, hi) are written (columns of hi - lo rows) and the carry is taken at rows->carry_row (-1: the carry passed in stays);
 // otherwise every row, and the carry at the last row.  The carry is replaced only on success.
@@ -881,12 +1042,50 @@ static std::vector<Column*> window_functions(WindowPlan& p, const Table* t, Wind
     return range_frames.back().second;
   };
 
-  ColsGuard outs;
+  // the rank directory of each distinct column that an IGNORE NULLS function reads and that has NULLs, shared likewise
+  std::vector<std::pair<int, DevBuf>> dirs;
+  auto dir_of = [&](int c) -> const int32_t* {
+    for (auto& d : dirs)
+      if (d.first == c) return d.second.as<int32_t>();
+    const int64_t nw = (n + 31) / 32;
+    DevBuf d((size_t)(nw + 1) * 4);
+    launch("window_valid_popc_kernel", window_valid_popc_kernel, grid_for(nw, 256), 256, 0, stream(), t->cols[c]->validity(), n, nw, d.as<int32_t>());
+    exclusive_scan<int32_t, int32_t>(d.as<int32_t>(), d.as<int32_t>(), nw, true);
+    dirs.emplace_back(c, std::move(d));
+    return dirs.back().second.as<int32_t>();
+  };
+
+  ColsGuard outs, next_value;
+  next_value.v.assign(nf + 1, nullptr);
   for (size_t k = 0; k < nf; k++) {
     const WinFn& f = p.fns[k];
     const int kind = f.s.kind;
     const DevBuf* cin = has_state && carry->state[k + 1].p ? &carry->state[k + 1] : nullptr;
     const Column* in = needs_column(kind) ? t->cols[f.s.column] : nullptr;
+    if (is_value_fn(kind)) {
+      const Column* cv = cin && k + 1 < carry->value.size() ? carry->value[k + 1] : nullptr;
+      const ValueFn vf{kind == B2_WIN_LAST ? 1 : 0, kind == B2_WIN_NTH_VALUE ? (int64_t)f.s.offset : 1, in->validity(),
+                       n && f.s.ignore_nulls && in->nullable() ? dir_of(f.s.column) : nullptr, n, cin ? cin->as<int64_t>() : nullptr};
+      const int32_t* s_at = nullptr;
+      if (f.frame == FR_RANGE_VALUE && n) s_at = frames_of(f).as<int32_t>();
+      const FrameArgs fr = frame_args(f);
+      DevBuf map((size_t)std::max<int64_t>(m, 1) * 4);
+      if (m && !rows)
+        launch("window_value_kernel", window_value_kernel<AllRows>, grid_for(n, 256), 256, 0, stream(), vf, fr, g, s_at, s_at ? s_at + n : nullptr,
+               AllRows{n}, map.as<int32_t>());
+      else if (m)
+        launch("window_value_kernel", window_value_kernel<RowRange>, grid_for(m, 256), 256, 0, stream(), vf, fr, g, s_at, s_at ? s_at + n : nullptr,
+               RowRange{lo, hi}, map.as<int32_t>());
+      outs.v.push_back(gather_values(t, f.s.column, map.as<int32_t>(), m, cv));
+      if (carry && n && carry_row >= 0) {
+        next_state[k + 1] = DevBuf(8);
+        DevBuf one(4);
+        launch("window_value_carry_kernel", window_value_carry_kernel, 1, 1, 0, stream(), vf, rank.as<RankOp::T>(), carry_row,
+               next_state[k + 1].as<int64_t>(), one.as<int32_t>());
+        next_value.v[k + 1] = gather_values(t, f.s.column, one.as<int32_t>(), 1, cv);
+      }
+      continue;
+    }
     if (is_offset_fn(kind)) {
       DevBuf map((size_t)std::max<int64_t>(m, 1) * 4);
       const int64_t off = kind == B2_WIN_LEAD ? (int64_t)f.s.offset : -(int64_t)f.s.offset;
@@ -942,6 +1141,8 @@ static std::vector<Column*> window_functions(WindowPlan& p, const Table* t, Wind
     if (carry->last) table_release(carry->last);
     carry->last = nl;
     carry->state = std::move(next_state);
+    for (Column* c : carry->value) if (c) col_release(c);
+    carry->value = next_value.release();
   }
   return outs.release();
 }

@@ -25,7 +25,13 @@ struct WindowPlan {
 struct WindowCarry {
   Table* last = nullptr;
   std::vector<DevBuf> state;   // [0] ranking, then one per function (empty where it has none)
-  ~WindowCarry() { if (last) table_release(last); }
+  // FIRST / LAST / NTH_VALUE, indexed as state (whose entry is then the int64 count of the open partition's rows so far that
+  // count): the one-row column of the value a continuing frame resolves to, or null
+  std::vector<Column*> value;
+  ~WindowCarry() {
+    if (last) table_release(last);
+    for (Column* c : value) if (c) col_release(c);
+  }
 };
 
 // checks the specs and classifies their frames (B2_ERR_INVALID / B2_ERR_UNSUPPORTED); bind_window checks the columns of a batch
