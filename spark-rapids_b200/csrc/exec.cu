@@ -77,6 +77,32 @@ struct TableRef {  // owning reference
 };
 
 static Table* from_handle_owned(b2_handle h) { return h ? reinterpret_cast<Table*>((intptr_t)h) : nullptr; }
+// raises the error of a failed b2_* call
+static void ok(int rc) {
+  if (rc != B2_OK) throw Error(rc, b2_last_error());
+}
+// one table of the batches `ts` (which it takes): the single batch, or their concatenation; null when there are none
+static Table* one_table(std::vector<TableRef> ts) {
+  if (ts.empty()) return nullptr;
+  if (ts.size() == 1) return ts[0].release();
+  std::vector<const Table*> v;
+  for (auto& t : ts) v.push_back(t.t);
+  return concat_tables(v);
+}
+// the columns of a then b in one table; steals them from both
+static Table* concat_cols(Table* a, Table* b) {
+  std::vector<Column*> cols;
+  for (auto*& c : a->cols) { cols.push_back(c); c = nullptr; }
+  for (auto*& c : b->cols) { cols.push_back(c); c = nullptr; }
+  a->cols.clear(); b->cols.clear();
+  return new_table(std::move(cols));
+}
+// n all-NULL rows of the columns `cols` of `schema` (null: all of them)
+static Table* null_rows(const Table* schema, int64_t n, const std::vector<int>* cols) {
+  ColGuard oob(new_column(B2_INT32, 0, n, false));
+  if (n) CUDA_CHECK(cudaMemsetAsync(oob.c->data.p, 0x80, (size_t)n * 4, stream()));   // 0x80808080 < 0: out of bounds -> NULL row
+  return gather_table(schema, oob.c->data.as<int32_t>(), n, true, cols);
+}
 
 // A batch waiting in the spill store, with the facts about it that planning needs, so that planning never brings it back
 struct SpillPiece {
@@ -96,14 +122,12 @@ struct SpillPiece {
   void hold(const Table* t) {
     rows = t->rows; bytes = table_bytes(t);
     for (const Column* c : t->cols) { chars.push_back(c->dtype == B2_STRING ? c->chars_bytes : 0); nullable.push_back(c->nullable()); }
-    int rc = b2_spillable_create(to_handle(const_cast<Table*>(t)), &sp);
-    if (rc != B2_OK) throw Error(rc, b2_last_error());
+    ok(b2_spillable_create(to_handle(const_cast<Table*>(t)), &sp));
   }
   void close() { if (sp) b2_spillable_close(sp); sp = 0; }
   Table* get() const {
     b2_handle h = 0;
-    int rc = b2_spillable_get(sp, &h);
-    if (rc != B2_OK) throw Error(rc, b2_last_error());
+    ok(b2_spillable_get(sp, &h));
     return from_handle_owned(h);
   }
 };
@@ -131,10 +155,8 @@ static Table* concat_pieces(const std::vector<SpillPiece>& ps, const Table* empt
   return with_retry([&]() -> Table* {
     if (ps.empty()) { Table* e = const_cast<Table*>(empty); e->refs.fetch_add(1); return e; }
     std::vector<TableRef> got;
-    std::vector<const Table*> ts;
-    for (auto& p : ps) { got.emplace_back(p.get()); ts.push_back(got.back().t); }
-    if (ts.size() == 1) return got[0].release();
-    return concat_tables(ts);
+    for (auto& p : ps) got.emplace_back(p.get());
+    return one_table(std::move(got));
   });
 }
 
@@ -165,9 +187,10 @@ struct GpuExec {
     Table* t = do_next();
     op_time_ns += std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now() - t0).count();
     if (prof) { cudaEventRecord(sp.b, stream()); spans.push_back(sp); if (parent) parent->child_spans.push_back(sp); }
-    if (t) { num_output_rows += t->rows; num_output_batches++; }
+    if (t) count(t->rows);
     return t;
   }
+  void count(int64_t rows) { num_output_rows += rows; num_output_batches++; }   // one output batch of `rows` rows
   // run f() as if node `who` had done it (an operator fused into this one keeps its own line in the metrics)
   template <typename F>
   auto run_as(GpuExec* who, F&& f) -> decltype(f()) {
@@ -186,6 +209,12 @@ struct GpuExec {
 static GpuExec* exec_from(b2_handle h) {
   if (!h) throw Error(B2_ERR_INVALID, "null exec handle");
   return reinterpret_cast<GpuExec*>((intptr_t)h);
+}
+// every batch `child` has left
+static std::vector<TableRef> pull_all(GpuExec* child) {
+  std::vector<TableRef> out;
+  while (Table* t = child->next()) out.emplace_back(t);
+  return out;
 }
 
 struct GpuBatchSource : GpuExec {
@@ -208,23 +237,40 @@ struct GpuParquetScanExec : GpuExec {
     std::vector<const char*> cn;
     for (auto& s : names) cn.push_back(s.c_str());
     b2_handle out = 0;
-    int rc = b2_parquet_decode(b.p, b.len, cn.data(), (int)cn.size(), &out);
-    if (rc != B2_OK) throw Error(rc, b2_last_error());
+    ok(b2_parquet_decode(b.p, b.len, cn.data(), (int)cn.size(), &out));
     return from_handle_owned(out);
   }
 };
 
+// A parent that fuses the filter (GpuShuffledHashJoinExec, GpuShuffleExchangeExec) pulls the filter's input batches itself and
+// uses the members below; the filter keeps its own line in the metrics.
 struct GpuFilterExec : GpuExec {
   b2_handle program;
   std::vector<int32_t> keep;   // non-empty: a column-pruning GpuProjectExec above the filter, fused (only these are compacted)
+  int input_col(int c) const { return keep.empty() ? c : keep[c]; }   // the input column of output column c
+  std::vector<int> input_cols(const Table* raw) const {               // the input column of every output column
+    std::vector<int> cols;
+    const int n = keep.empty() ? (int)raw->cols.size() : (int)keep.size();
+    for (int c = 0; c < n; c++) cols.push_back(input_col(c));
+    return cols;
+  }
+  // the selection vector of input batch `raw`, timed as this node inside the parent running it; counted: this node's output
+  // metrics take the batch
+  Column* row_ids(const Table* raw, bool counted = true) {
+    Column* sel = current()->run_as(this, [&] { return filter_row_ids(program_from(program), raw); });
+    if (counted) count(sel->size);
+    return sel;
+  }
+  // the filter's output for input batch `raw`
+  Table* apply(const Table* raw) {
+    if (!keep.empty()) return filter_select(program_from(program), raw, keep.data(), (int)keep.size());
+    b2_handle out = 0;
+    ok(b2_filter(program, to_handle(const_cast<Table*>(raw)), &out));
+    return from_handle_owned(out);
+  }
   Table* do_next() override {
     TableRef in(children[0]->next());
-    if (!in.t) return nullptr;
-    if (!keep.empty()) return filter_select(program_from(program), in.t, keep.data(), (int)keep.size());
-    b2_handle out = 0;
-    int rc = b2_filter(program, to_handle(in.t), &out);
-    if (rc != B2_OK) throw Error(rc, b2_last_error());
-    return from_handle_owned(out);
+    return in.t ? apply(in.t) : nullptr;
   }
 };
 
@@ -306,8 +352,7 @@ struct GpuProjectExec : GpuExec {
     TableRef in(children[0]->next());
     if (!in.t) return nullptr;
     b2_handle out = 0;
-    int rc = b2_project(program, to_handle(in.t), &out);
-    if (rc != B2_OK) throw Error(rc, b2_last_error());
+    ok(b2_project(program, to_handle(in.t), &out));
     return from_handle_owned(out);
   }
 };
@@ -322,14 +367,10 @@ struct GpuExpandExec : GpuExec {
     std::vector<TableRef> parts;
     for (b2_handle p : projections) {
       b2_handle out = 0;
-      int rc = b2_project(p, to_handle(in.t), &out);
-      if (rc != B2_OK) throw Error(rc, b2_last_error());
+      ok(b2_project(p, to_handle(in.t), &out));
       parts.emplace_back(from_handle_owned(out));
     }
-    if (parts.size() == 1) return parts[0].release();
-    std::vector<const Table*> ts;
-    for (auto& p : parts) ts.push_back(p.t);
-    return concat_tables(ts);
+    return one_table(std::move(parts));
   }
 };
 
@@ -476,9 +517,7 @@ struct GpuHashAggregateExec : GpuExec {
       throw Error(B2_ERR_UNSUPPORTED, "keyless aggregate over zero input batches needs the input schema");
     }
     if (partials.size() == 1 && mode != B2_AGG_MODE_FINAL) return without_counts(partials[0].release());
-    std::vector<const Table*> ts;
-    for (auto& p : partials) ts.push_back(p.t);
-    TableRef cat(concat_tables(ts));
+    TableRef cat(one_table(std::move(partials)));
     return merge(cat.t);
   }
 
@@ -621,7 +660,9 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
   // the hash table keeps the build rows that found a partner, and once the stream side is exhausted the others come out
   // with NULL stream columns (getFinalBatch, :2288-2326).  FULL OUTER without a condition coalesces its stream side instead.
   b2_handle tracker = 0;
-  TableRef stream_schema;                       // zero rows of the stream columns: the NULL side of the final rows
+  // zero rows of the stream side as the join sees it, which stream_out indexes (the filter's output when one is fused, the carried
+  // columns when sub-partitioned): the NULL side of the final rows, and the schema of a sub-partition pair without stream rows
+  TableRef stream_schema;
   Column* fin_ids = nullptr;                    // ascending ids of the unmatched build rows
   std::deque<std::pair<int64_t, int64_t>> fin;  // ranges of fin_ids still to emit
   bool fin_started = false;
@@ -632,19 +673,25 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
   }
   bool tracked() const { return kind == B2_JOIN_RIGHT_OUTER || (kind == B2_JOIN_FULL_OUTER && condition); }
   bool coalesced() const { return kind == B2_JOIN_FULL_OUTER && !condition; }
-  void new_tracker() {   // after (re)building ht
+  // the hash table over build_table's keys and, for a tracked join, its tracker (retry: the build of the table runs under
+  // with_retry)
+  void build_hash(bool retry) {
+    auto make = [&] {
+      TableRef bk(select(build_table.t, build_keys));
+      b2_handle h = 0;
+      ok(b2_join_build(to_handle(bk.t), nulls_equal, &h));
+      return h;
+    };
+    ht = retry ? with_retry(make) : make();
     if (tracker) { b2_join_tracker_close(tracker); tracker = 0; }
     fin_started = false;
-    if (!tracked()) return;
-    int rc = b2_join_tracker_create(ht, &tracker);
-    if (rc != B2_OK) throw Error(rc, b2_last_error());
+    if (tracked()) ok(b2_join_tracker_create(ht, &tracker));
   }
   // the maps of one stream batch (through a selection vector): RIGHT OUTER probes INNER and marks the build rows it finds
   void probe(const Table* keys, Column* sel, b2_handle* lm, b2_handle* rm) {
     const b2_handle sh = sel ? to_handle(sel) : 0;
-    int rc = kind == B2_JOIN_RIGHT_OUTER ? b2_join_probe_track(ht, to_handle(const_cast<Table*>(keys)), sh, B2_JOIN_INNER, tracker, lm, rm)
-                                         : b2_join_probe_sel(ht, to_handle(const_cast<Table*>(keys)), sh, kind, lm, rm);
-    if (rc != B2_OK) throw Error(rc, b2_last_error());
+    ok(kind == B2_JOIN_RIGHT_OUTER ? b2_join_probe_track(ht, to_handle(const_cast<Table*>(keys)), sh, B2_JOIN_INNER, tracker, lm, rm)
+                                   : b2_join_probe_sel(ht, to_handle(const_cast<Table*>(keys)), sh, kind, lm, rm));
   }
   static Table* select(const Table* t, const std::vector<int>& idx) {
     std::vector<Column*> cols;
@@ -657,24 +704,24 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
     if (sp_target > 0) {
       if (hold_build_side(parts)) { built = true; return; }
     } else {
-      while (true) { TableRef b(children[1]->next()); if (!b.t) break; parts.emplace_back(b.release()); }
+      parts = pull_all(children[1]);
     }
-    if (parts.empty()) throw Error(B2_ERR_UNSUPPORTED, "empty build side needs the build schema");
-    if (parts.size() == 1) build_table = std::move(parts[0]);
-    else { std::vector<const Table*> ts; for (auto& p : parts) ts.push_back(p.t); build_table = TableRef(concat_tables(ts)); }
-    parts.clear();   // the batches are not needed once concatenated: the hash table does not wait for them to go
-    TableRef bk(select(build_table.t, build_keys));
-    int rc = b2_join_build(to_handle(bk.t), nulls_equal, &ht);
-    if (rc != B2_OK) throw Error(rc, b2_last_error());
-    new_tracker();
+    // the batches go once concatenated: the hash table does not wait for them
+    build_table = TableRef(one_table(std::move(parts)));
+    if (!build_table.t) throw Error(B2_ERR_UNSUPPORTED, "empty build side needs the build schema");
+    build_hash(false);
     built = true;
   }
   // A GpuFilterExec directly below the stream side is fused by late materialisation: the filter yields a selection vector
   // (row ids), the probe reads the keys through it and emits ORIGINAL row ids, the payload is gathered from the unfiltered
   // batch — the filtered copy of the stream side (TPC-H q3: 7.8 GB per pass over lineitem) is never written or re-read.
   GpuFilterExec* fused = nullptr;
-  bool fusion_checked = false;
-  int raw_col(int filter_out_col) const { return fused->keep.empty() ? filter_out_col : fused->keep[filter_out_col]; }
+  GpuFilterExec* fusable_filter() const {
+    if (kind == B2_JOIN_FULL_OUTER || condition || getenv("B2_NO_FILTER_FUSION")) return nullptr;
+    return dynamic_cast<GpuFilterExec*>(children[0]);
+  }
+  // fused: the filter's input columns of the stream keys, of the stream columns joined and of every filter output
+  std::vector<int> f_keys, f_stream, f_all;
   // Emitting probe (join_probe_pred_emit): the maps and the payload gathers of a filtered FK -> PK join replaced by output rows
   // written from the probe kernel.  The output size is known only after the probe, and GpuCoalesceBatches above holds every
   // output batch, so columns of the batch's row count are out of the question: the first batch goes through the maps and
@@ -708,32 +755,29 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
   Table* fused_next() {
     TableRef raw(fused->children[0]->next());
     if (!raw.t) return nullptr;
-    std::vector<int> keys, left_cols;
-    for (int k : stream_keys) keys.push_back(raw_col(k));
+    if (f_keys.empty()) {   // the first batch (a join has at least one key)
+      f_all = fused->input_cols(raw.t);
+      for (int k : stream_keys) f_keys.push_back(fused->input_col(k));
+      if (pruned) for (int c : stream_out) f_stream.push_back(fused->input_col(c));
+      else f_stream = f_all;
+      if (tracked()) { TableRef cols(select(raw.t, f_all)); stream_schema = TableRef(slice_table(cols.t, 0, 0)); }
+    }
     // simple predicate + FK -> PK inner probe: the filter is evaluated INSIDE the probe kernel (no selection vector at all)
     struct Owned { Column* c = nullptr; ~Owned() { if (c) col_release(c); } Column* take() { Column* r = c; c = nullptr; return r; } };
     Owned plm, prm, sel;
     int64_t npass = 0;
     bool in_probe = false;
-    if (tracked() && !stream_schema.t) {
-      std::vector<int> fcols;
-      const int n = fused->keep.empty() ? (int)raw.t->cols.size() : (int)fused->keep.size();
-      for (int c = 0; c < n; c++) fcols.push_back(raw_col(c));
-      TableRef cols(select(raw.t, fcols));
-      stream_schema = TableRef(slice_table(cols.t, 0, 0));
-    }
-    if (pruned) for (int c : stream_out) left_cols.push_back(raw_col(c));
-    else { const int n = fused->keep.empty() ? (int)raw.t->cols.size() : (int)fused->keep.size(); for (int c = 0; c < n; c++) left_cols.push_back(raw_col(c)); }
     TableRef emitted;
-    if ((kind == B2_JOIN_INNER || kind == B2_JOIN_RIGHT_OUTER) && keys.size() == 1) {
+    if ((kind == B2_JOIN_INNER || kind == B2_JOIN_RIGHT_OUTER) && f_keys.size() == 1) {
       try {
-        emitted = TableRef(try_emit(raw.t, keys[0], left_cols, &npass));
-        if (!emitted.t) in_probe = join_probe_pred(ht, raw.t, keys[0], program_from(fused->program), &plm.c, &prm.c, &npass, tracker);
+        emitted = TableRef(try_emit(raw.t, f_keys[0], f_stream, &npass));
+        if (!emitted.t) in_probe = join_probe_pred(ht, raw.t, f_keys[0], program_from(fused->program), &plm.c, &prm.c, &npass, tracker);
       } catch (const Error& e) { if (!splittable(e)) throw; in_probe = false; }   // memory pressure: the selection-vector path retries and splits
     }
-    auto make_sel = [&] { if (!sel.c) sel.c = run_as(fused, [&] { return filter_row_ids(program_from(fused->program), raw.t); }); };
-    if (!in_probe && !emitted.t) make_sel();
-    fused->num_output_rows += in_probe || emitted.t ? npass : sel.c->size; fused->num_output_batches++;
+    if (in_probe || emitted.t) fused->count(npass);
+    else sel.c = fused->row_ids(raw.t);
+    // the selection vector after all (the in-probe maps were lost to a retry or a split): the filter has counted this batch
+    auto make_sel = [&] { if (!sel.c) sel.c = fused->row_ids(raw.t, false); };
     if (emitted.t) { em_stats[0]++; return emitted.release(); }
     try {
       Table* out = with_retry([&]() -> Table* {
@@ -741,7 +785,7 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
         if (plm.c) { lmc = plm.take(); rmc = prm.take(); }   // the maps of the fused kernel (first attempt only)
         else {
           make_sel();
-          TableRef sk(select(raw.t, keys));
+          TableRef sk(select(raw.t, f_keys));
           b2_handle lm = 0, rm = 0;
           probe(sk.t, sel.c, &lm, &rm);
           lmc = col_from(lm); rmc = rm ? col_from(rm) : nullptr;
@@ -749,26 +793,15 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
         ColGuard lmap(lmc);
         ColGuard rmap(rmc);
         note_matches(lmap.c->size, raw.t->rows);
-        TableRef left(gather_table(raw.t, lmap.c->data.as<int32_t>(), lmap.c->size, false, &left_cols));
-        if (!rmap.c || (pruned && build_out.empty())) return left.release();
-        TableRef right(gather_table(build_table.t, rmap.c->data.as<int32_t>(), rmap.c->size, kind == B2_JOIN_LEFT_OUTER, pruned ? &build_out : nullptr));
-        if (pruned && stream_out.empty()) return right.release();
-        std::vector<Column*> cols;
-        for (auto*& c : left.t->cols) { cols.push_back(c); c = nullptr; }
-        for (auto*& c : right.t->cols) { cols.push_back(c); c = nullptr; }
-        left.t->cols.clear(); right.t->cols.clear();
-        return new_table(std::move(cols));
+        return joined_rows(raw.t, lmap.c, rmap.c, &f_stream);
       });
       em_stats[1]++;
       return out;
     } catch (const Error& e) {
       if (!splittable(e)) throw;
       // memory pressure / 2^31 limit: materialise the filter output after all and take the split-and-retry path
-      std::vector<int> fcols;
-      const int n = fused->keep.empty() ? (int)raw.t->cols.size() : (int)fused->keep.size();
-      for (int c = 0; c < n; c++) fcols.push_back(raw_col(c));
       make_sel();
-      TableRef ft(gather_table(raw.t, sel.c->data.as<int32_t>(), sel.c->size, false, &fcols));
+      TableRef ft(gather_table(raw.t, sel.c->data.as<int32_t>(), sel.c->size, false, &f_all));
       todo.emplace_back(std::move(ft), 0);
       return drain_todo();
     }
@@ -776,12 +809,8 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
   Table* do_next() override {
     if (!todo.empty()) return drain_todo();
     if (!fin.empty()) return final_next();
-    if (!built) build();
+    if (!built) { build(); fused = fusable_filter(); }
     if (sp_active) return sp_next();
-    if (!fusion_checked) {
-      fusion_checked = true;
-      if (kind != B2_JOIN_FULL_OUTER && !condition && !getenv("B2_NO_FILTER_FUSION")) fused = dynamic_cast<GpuFilterExec*>(children[0]);
-    }
     if (fused) {
       if (Table* t = fused_next()) return t;
       return tracked() ? final_start() : nullptr;
@@ -792,11 +821,8 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
       // side is coalesced into one batch (tracked joins keep the matched build rows across batches instead: final_start)
       if (full_done) return nullptr;
       full_done = true;
-      std::vector<TableRef> parts;
-      while (true) { TableRef b(children[0]->next()); if (!b.t) break; parts.emplace_back(b.release()); }
-      if (parts.empty()) throw Error(B2_ERR_UNSUPPORTED, "empty stream side of a full outer join needs the stream schema");
-      if (parts.size() == 1) s = std::move(parts[0]);
-      else { std::vector<const Table*> ts; for (auto& q : parts) ts.push_back(q.t); s = TableRef(concat_tables(ts)); }
+      s = TableRef(one_table(pull_all(children[0])));
+      if (!s.t) throw Error(B2_ERR_UNSUPPORTED, "empty stream side of a full outer join needs the stream schema");
     } else {
       s = TableRef(children[0]->next());
     }
@@ -811,13 +837,11 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
   Table* final_start() {
     if (fin_started) return nullptr;
     fin_started = true;
-    if (!(sp_active ? sp_stream_empty.t : stream_schema.t))
-      throw Error(B2_ERR_UNSUPPORTED, "empty stream side of an outer join that preserves the build side needs the stream schema");
+    if (!stream_schema.t) throw Error(B2_ERR_UNSUPPORTED, "empty stream side of an outer join that preserves the build side needs the stream schema");
     if (fin_ids) { col_release(fin_ids); fin_ids = nullptr; }
     fin_ids = with_retry([&] {
       b2_handle h = 0;
-      int rc = b2_join_tracker_unmatched(tracker, &h);
-      if (rc != B2_OK) throw Error(rc, b2_last_error());
+      ok(b2_join_tracker_unmatched(tracker, &h));
       return col_from(h);
     });
     if (fin_ids->size) fin.emplace_back(0, fin_ids->size);
@@ -839,14 +863,8 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
     }
   }
   Table* final_rows(int64_t lo, int64_t hi) {
-    const Table* ss = sp_active ? sp_stream_empty.t : stream_schema.t;
     const int64_t n = hi - lo;
-    std::vector<int> scols;
-    if (pruned) scols = stream_out;
-    else for (int c = 0; c < (int)ss->cols.size(); c++) scols.push_back(c);
-    ColGuard oob(new_column(B2_INT32, 0, n, false));
-    if (n) CUDA_CHECK(cudaMemsetAsync(oob.c->data.p, 0x80, (size_t)n * 4, stream()));   // 0x80808080 < 0: out of bounds -> NULL row
-    TableRef left(gather_table(ss, oob.c->data.as<int32_t>(), n, true, &scols));
+    TableRef left(null_rows(stream_schema.t, n, pruned ? &stream_out : nullptr));
     TableRef right(gather_table(build_table.t, fin_ids->data.as<int32_t>() + lo, n, false, pruned ? &build_out : nullptr));
     return concat_cols(left.t, right.t);
   }
@@ -868,14 +886,8 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
         if (!splittable(e) || st.t->rows < 2 || depth >= 16 || coalesced()) throw;
         note_split();
         const int64_t mid = st.t->rows / 2;
-        TableRef lo, hi;
         // the halves replace the batch: the batch itself is released before they are made, so the split needs no extra room
-        {
-          std::vector<int> all;
-          for (int c = 0; c < (int)st.t->cols.size(); c++) all.push_back(c);
-          lo = TableRef(slice_table(st.t, 0, mid));
-          hi = TableRef(slice_table(st.t, mid, st.t->rows));
-        }
+        TableRef lo(slice_table(st.t, 0, mid)), hi(slice_table(st.t, mid, st.t->rows));
         st.reset();
         todo.emplace_front(std::move(hi), depth + 1);
         todo.emplace_front(std::move(lo), depth + 1);
@@ -883,12 +895,15 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
     }
     return nullptr;
   }
-  static Table* concat_cols(Table* a, Table* b) {   // steals the columns of both
-    std::vector<Column*> cols;
-    for (auto*& c : a->cols) { cols.push_back(c); c = nullptr; }
-    for (auto*& c : b->cols) { cols.push_back(c); c = nullptr; }
-    a->cols.clear(); b->cols.clear();
-    return new_table(std::move(cols));
+  // the output rows of stream batch `st` (its columns `scols`; null: all) from the gather maps: stream columns ++ build columns
+  // (GpuHashJoin.scala:2451-2470).  Without a right map (semi / anti) or anything wanted from the build side: the stream columns.
+  Table* joined_rows(const Table* st, const Column* lmap, const Column* rmap, const std::vector<int>* scols) {
+    TableRef left(gather_table(st, lmap->data.as<int32_t>(), lmap->size, kind == B2_JOIN_FULL_OUTER, scols));
+    if (!rmap || (pruned && build_out.empty())) return left.release();
+    TableRef right(gather_table(build_table.t, rmap->data.as<int32_t>(), rmap->size, kind == B2_JOIN_LEFT_OUTER || kind == B2_JOIN_FULL_OUTER,
+                                pruned ? &build_out : nullptr));
+    if (pruned && stream_out.empty()) return right.release();
+    return concat_cols(left.t, right.t);
   }
   Table* prune_pairs(const Table* pairs, int nstream) {   // [stream ++ build] -> the output columns of the node
     std::vector<Column*> cols;
@@ -901,23 +916,19 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
   Table* join_batch_conditional(const Table* st) {
     TableRef sk(select(st, stream_keys));
     b2_handle lm = 0, rm = 0;
-    int rc = b2_join_probe(ht, to_handle(sk.t), B2_JOIN_INNER, &lm, &rm);
-    if (rc != B2_OK) throw Error(rc, b2_last_error());
+    ok(b2_join_probe(ht, to_handle(sk.t), B2_JOIN_INNER, &lm, &rm));
     ColGuard lmap(col_from(lm)), rmap(col_from(rm));
     const int nstream = (int)st->cols.size();
     TableRef left(gather_table(st, lmap.c->data.as<int32_t>(), lmap.c->size, false, nullptr));
     TableRef right(gather_table(build_table.t, rmap.c->data.as<int32_t>(), rmap.c->size, false, nullptr));
     TableRef pairs(concat_cols(left.t, right.t));
     b2_handle ph = 0;
-    rc = b2_project(condition, to_handle(pairs.t), &ph);
-    if (rc != B2_OK) throw Error(rc, b2_last_error());
+    ok(b2_project(condition, to_handle(pairs.t), &ph));
     TableRef pt(from_handle_owned(ph));
     Column* pass = pt.t->cols[0];
     if (pass->dtype != B2_BOOL8) throw Error(B2_ERR_INVALID, "join condition must be BOOL8");
-    if (tracker) {   // the build rows of the pairs that pass (marking is idempotent: a retried or halved batch sets the same bits)
-      rc = b2_join_tracker_mark(tracker, to_handle(rmap.c), to_handle(pass));
-      if (rc != B2_OK) throw Error(rc, b2_last_error());
-    }
+    // the build rows of the pairs that pass (marking is idempotent: a retried or halved batch sets the same bits)
+    if (tracker) ok(b2_join_tracker_mark(tracker, to_handle(rmap.c), to_handle(pass)));
     auto stream_side = [&](const Table* t) {   // semi / anti output: the node's stream columns
       std::vector<Column*> cols;
       if (pruned) for (int c : stream_out) { col_incref(t->cols[c]); cols.push_back(t->cols[c]); }
@@ -938,9 +949,7 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
     TableRef matched(filter_by_mask(pruned_pairs.t, pass));
     ColGuard lonely(rows_with_passing_pair(lmap.c, pass, st->rows, true));
     TableRef lonely_stream(filter_by_mask(st, lonely.c));
-    ColGuard oob(new_column(B2_INT32, 0, lonely_stream.t->rows, false));
-    if (lonely_stream.t->rows) CUDA_CHECK(cudaMemsetAsync(oob.c->data.p, 0x80, (size_t)lonely_stream.t->rows * 4, stream()));   // 0x80808080 < 0: out of bounds -> NULL row
-    TableRef nulls(gather_table(build_table.t, oob.c->data.as<int32_t>(), lonely_stream.t->rows, true, nullptr));
+    TableRef nulls(null_rows(build_table.t, lonely_stream.t->rows, nullptr));
     TableRef lonely_pairs(concat_cols(lonely_stream.t, nulls.t));
     TableRef lonely_out(prune_pairs(lonely_pairs.t, nstream));
     // nullability must agree for the concatenation: concat_tables merges validity
@@ -954,16 +963,7 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
     probe(sk.t, nullptr, &lm, &rm);
     ColGuard lmap(col_from(lm));
     ColGuard rmap(rm ? col_from(rm) : nullptr);
-    TableRef left(gather_table(st, lmap.c->data.as<int32_t>(), lmap.c->size, kind == B2_JOIN_FULL_OUTER, pruned ? &stream_out : nullptr));
-    if (!rmap.c || (pruned && build_out.empty())) return left.release();  // semi / anti (or nothing wanted from the build side): stream columns only
-    TableRef right(gather_table(build_table.t, rmap.c->data.as<int32_t>(), rmap.c->size, kind == B2_JOIN_LEFT_OUTER || kind == B2_JOIN_FULL_OUTER,
-                                pruned ? &build_out : nullptr));
-    if (pruned && stream_out.empty()) return right.release();
-    std::vector<Column*> cols;  // output = left columns ++ right columns (GpuHashJoin.scala:2451-2470)
-    for (auto*& c : left.t->cols) { cols.push_back(c); c = nullptr; }
-    for (auto*& c : right.t->cols) { cols.push_back(c); c = nullptr; }
-    left.t->cols.clear(); right.t->cols.clear();
-    return new_table(std::move(cols));
+    return joined_rows(st, lmap.c, rmap.c, pruned ? &stream_out : nullptr);
   }
 
   // ---- GpuSubPartitionHashJoin (GpuSubPartitionHashJoin.scala) -------------------------------------------------------------
@@ -981,7 +981,7 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
   };
   std::deque<Bucket> sp_buckets;
   std::deque<std::vector<SpillPiece>> sp_probe;   // the open pair's stream pieces, one group per probe batch
-  TableRef sp_build_empty, sp_stream_empty;       // zero-row tables of the carried columns
+  TableRef sp_build_empty;                        // zero rows of the carried build columns
   std::vector<int> sp_bkeys, sp_bkeep;            // first-level split of the build batches: keys and carried columns
 
   // the columns one side carries through its buckets: with pruning and no condition the keys and the output columns (indices
@@ -1044,27 +1044,24 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
   }
   // The stream side, split by the same keys, seed and K; through the selection vector of a GpuFilterExec directly below
   void split_stream_side() {
-    GpuFilterExec* ff = nullptr;
-    if (kind != B2_JOIN_FULL_OUTER && !condition && !getenv("B2_NO_FILTER_FUSION")) ff = dynamic_cast<GpuFilterExec*>(children[0]);
     std::vector<int> keys, keep;   // indices into the batches pulled (the filter's input when fused)
     auto first_level = [&](int p) -> Bucket& { return sp_buckets[p]; };
     while (true) {
-      TableRef raw(ff ? ff->children[0]->next() : children[0]->next());
+      TableRef raw(fused ? fused->children[0]->next() : children[0]->next());
       if (!raw.t) break;
       if (keep.empty()) {
-        const int ncols = ff && !ff->keep.empty() ? (int)ff->keep.size() : (int)raw.t->cols.size();
-        auto raw_of = [&](int c) { return ff && !ff->keep.empty() ? ff->keep[c] : c; };
+        const int ncols = fused ? (int)fused->input_cols(raw.t).size() : (int)raw.t->cols.size();
+        auto raw_of = [&](int c) { return fused ? fused->input_col(c) : c; };
         for (int k : stream_keys) keys.push_back(raw_of(k));
         for (int c : carried(ncols, stream_keys, stream_out)) keep.push_back(raw_of(c));
         TableRef sel(select(raw.t, keep));
-        sp_stream_empty = TableRef(slice_table(sel.t, 0, 0));
+        stream_schema = TableRef(slice_table(sel.t, 0, 0));
       }
-      ColGuard sel(ff ? run_as(ff, [&] { return filter_row_ids(program_from(ff->program), raw.t); }) : nullptr);
-      if (ff) { ff->num_output_rows += sel.c->size; ff->num_output_batches++; }
+      ColGuard sel(fused ? fused->row_ids(raw.t) : nullptr);
       split_into(raw.t, sel.c ? sel.c->data.as<int32_t>() : nullptr, sel.c ? sel.c->size : raw.t->rows, keys, keep, SP_SEED, sp_parts,
                  first_level, false, &sp_stats[3]);
     }
-    if (!sp_stream_empty.t && (coalesced() || tracked()))
+    if (!stream_schema.t && (coalesced() || tracked()))
       throw Error(B2_ERR_UNSUPPORTED, "empty stream side of an outer join that preserves the build side needs the stream schema");
   }
   bool useless(const Bucket& b) const {
@@ -1085,7 +1082,7 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
     auto second_level = [&](int p) -> Bucket& { return sub[p]; };
     std::vector<int> all_b, all_s;
     for (int c = 0; c < (int)sp_build_empty.t->cols.size(); c++) all_b.push_back(c);
-    for (int c = 0; sp_stream_empty.t && c < (int)sp_stream_empty.t->cols.size(); c++) all_s.push_back(c);
+    for (int c = 0; stream_schema.t && c < (int)stream_schema.t->cols.size(); c++) all_s.push_back(c);
     for (auto& p : b.build) { TableRef t(with_retry([&] { return p.get(); })); p.close(); split_into(t.t, nullptr, t.t->rows, build_keys, all_b, SP_RESEED, k2, second_level, true, nullptr); }
     for (auto& p : b.stream) { TableRef t(with_retry([&] { return p.get(); })); p.close(); split_into(t.t, nullptr, t.t->rows, stream_keys, all_s, SP_RESEED, k2, second_level, false, nullptr); }
     for (int p = k2 - 1; p >= 0; p--) { sub[p].resplit = true; sp_buckets.push_front(std::move(sub[p])); }
@@ -1127,14 +1124,7 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
     }
     build_table = TableRef(concat_pieces(bp, sp_build_empty.t));
     bp.clear();
-    ht = with_retry([&] {
-      TableRef bk(select(build_table.t, build_keys));
-      b2_handle h = 0;
-      int rc = b2_join_build(to_handle(bk.t), nulls_equal, &h);
-      if (rc != B2_OK) throw Error(rc, b2_last_error());
-      return h;
-    });
-    new_tracker();
+    build_hash(true);
     if (full) { sp_probe.push_back(std::move(sps)); return true; }
     std::vector<SpillPiece> grp;
     int64_t gb = 0, gr = 0;
@@ -1154,7 +1144,7 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
       if (!sp_probe.empty()) {
         std::vector<SpillPiece> grp = std::move(sp_probe.front());
         sp_probe.pop_front();
-        todo.emplace_back(TableRef(concat_pieces(grp, sp_stream_empty.t)), 0);
+        todo.emplace_back(TableRef(concat_pieces(grp, stream_schema.t)), 0);
         continue;
       }
       if (ht && tracked() && !fin_started) {   // the pair's last group is done (or it had none): its unmatched build rows
@@ -1185,28 +1175,20 @@ struct GpuSortExec : GpuExec {
     }
     if (done) return nullptr;
     done = true;
+    if (limit < 0) {   // full sort: every batch, concatenated once
+      TableRef all(one_table(pull_all(children[0])));
+      return all.t ? sorted(all.t, -1) : nullptr;
+    }
     TableRef pending;
-    std::vector<TableRef> all;   // full sort: every batch, concatenated once
     while (true) {
       TableRef in(children[0]->next());
       if (!in.t) break;
-      if (limit >= 0) {
-        // GpuTopN: sort the batch, keep N, fold into the running top-N
-        TableRef top(sorted(in.t, limit));
-        if (!pending.t) pending = std::move(top);
-        else { std::vector<const Table*> ts{pending.t, top.t}; TableRef cat(concat_tables(ts)); pending = TableRef(sorted(cat.t, limit)); }
-      } else {
-        all.push_back(std::move(in));
-      }
+      // GpuTopN: sort the batch, keep N, fold into the running top-N
+      TableRef top(sorted(in.t, limit));
+      if (!pending.t) pending = std::move(top);
+      else { std::vector<const Table*> ts{pending.t, top.t}; TableRef cat(concat_tables(ts)); pending = TableRef(sorted(cat.t, limit)); }
     }
-    if (limit >= 0) return pending.release();
-    if (all.empty()) return nullptr;
-    if (all.size() == 1) return sorted(all[0].t, -1);
-    std::vector<const Table*> ts;
-    for (auto& a : all) ts.push_back(a.t);
-    TableRef cat(concat_tables(ts));
-    all.clear();
-    return sorted(cat.t, -1);
+    return pending.release();
   }
 };
 
@@ -1393,10 +1375,7 @@ struct GpuOutOfCoreSortExec : GpuExec {
         for (Column* c : cols) col_incref(c);
         parts.emplace_back(new_table(std::move(cols)));
       }
-      if (n == 1) return parts[0].release();
-      std::vector<const Table*> ts;
-      for (auto& p : parts) ts.push_back(p.t);
-      return concat_tables(ts);
+      return one_table(std::move(parts));
     });
     for (size_t i = 0; i < n; i++) { final_bytes -= final_q.front().bytes; final_q.pop_front(); }
     return out;
@@ -1599,11 +1578,7 @@ struct GpuCoalesceBatches : GpuExec {
       rows += in.t->rows;
       acc.emplace_back(in.release());
     }
-    if (acc.empty()) return nullptr;
-    if (acc.size() == 1) return acc[0].release();
-    std::vector<const Table*> ts;
-    for (auto& a : acc) ts.push_back(a.t);
-    return concat_tables(ts);
+    return one_table(std::move(acc));
   }
 };
 
@@ -1632,8 +1607,7 @@ struct GpuShuffleExchangeExec : GpuExec {
       if (key_cols.empty()) return in.release();
       std::vector<int32_t> offs(world + 1, 0);
       b2_handle out = 0;
-      int rc = b2_hash_partition(to_handle(in.t), key_cols.data(), (int)key_cols.size(), 42, world, &out, offs.data());
-      if (rc != B2_OK) throw Error(rc, b2_last_error());
+      ok(b2_hash_partition(to_handle(in.t), key_cols.data(), (int)key_cols.size(), 42, world, &out, offs.data()));
       return from_handle_owned(out);
     }
     // a GpuFilterExec (with its column pruning) directly below is fused into the scatter: see GpuShuffledHashJoinExec::fused
@@ -1644,47 +1618,34 @@ struct GpuShuffleExchangeExec : GpuExec {
     if (!primed) { primed = true; ahead = TableRef(src->next()); }
     TableRef in = std::move(ahead);
     if (in.t) ahead = TableRef(src->next());
-    {
-      int rc = b2_comm_set_more(comm, ahead.t ? 1 : 0);
-      if (rc != B2_OK) throw Error(rc, b2_last_error());
-    }
+    ok(b2_comm_set_more(comm, ahead.t ? 1 : 0));
     std::vector<int32_t> out_cols;     // the columns that travel (indices into the batch pulled from src)
-    if (ff && in.t) {
-      if (ff->keep.empty()) for (int c = 0; c < (int)in.t->cols.size(); c++) out_cols.push_back(c);
-      else out_cols = ff->keep;
-    }
+    if (ff && in.t) out_cols = ff->input_cols(in.t);
     if (!probed) {   // collective, once per node: can every rank store into every peer's arena, and is the schema fixed width?
-      int32_t ok = 0;
-      int rc = b2_comm_fused_ready(comm, &ok);
-      if (rc != B2_OK) throw Error(rc, b2_last_error());
+      int32_t ready = 0;
+      ok(b2_comm_fused_ready(comm, &ready));
       // a rank without a batch does not know the schema, so the ranks agree on "some batch carries STRING columns"
       int32_t mine = 0, any_strings = 0;
       if (in.t && !ff) for (auto* c : in.t->cols) if (c->dtype == B2_STRING) mine = 1;
       if (in.t && ff) for (int c : out_cols) if (in.t->cols[c]->dtype == B2_STRING) mine = 1;
-      rc = b2_comm_allmax(comm, mine, &any_strings);
-      if (rc != B2_OK) throw Error(rc, b2_last_error());
+      ok(b2_comm_allmax(comm, mine, &any_strings));
       has_strings = any_strings != 0;
-      fused = ok != 0; probed = true;
+      fused = ready != 0; probed = true;
     }
     b2_handle out = 0;
     int32_t any = 0;
     if (fused && !has_strings && ff) {
-      ColGuard sel(in.t ? run_as(ff, [&] { return filter_row_ids(program_from(ff->program), in.t); }) : nullptr);
-      if (in.t) { ff->num_output_rows += sel.c->size; ff->num_output_batches++; }
+      ColGuard sel(in.t ? ff->row_ids(in.t) : nullptr);
       std::vector<int32_t> keys;   // key_cols index the filter's output columns
-      for (int32_t k : key_cols) keys.push_back(ff->keep.empty() ? k : ff->keep[k]);
-      int rc = b2_exchange_hash_sel(comm, in.t ? to_handle(in.t) : 0, sel.c ? to_handle(sel.c) : 0, out_cols.data(), (int)out_cols.size(), keys.data(),
-                                    (int)keys.size(), 42, &out, &any);
-      if (rc != B2_OK) throw Error(rc, b2_last_error());
+      for (int32_t k : key_cols) keys.push_back(ff->input_col(k));
+      ok(b2_exchange_hash_sel(comm, in.t ? to_handle(in.t) : 0, sel.c ? to_handle(sel.c) : 0, out_cols.data(), (int)out_cols.size(), keys.data(),
+                              (int)keys.size(), 42, &out, &any));
     } else if (fused && !has_strings) {
-      int rc = b2_exchange_hash(comm, in.t ? to_handle(in.t) : 0, key_cols.data(), (int)key_cols.size(), 42, &out, &any);
-      if (rc != B2_OK) throw Error(rc, b2_last_error());
+      ok(b2_exchange_hash(comm, in.t ? to_handle(in.t) : 0, key_cols.data(), (int)key_cols.size(), 42, &out, &any));
     } else {
       if (ff && in.t) {   // NCCL path: the filter runs unfused
-        TableRef f(ff->keep.empty() ? nullptr : filter_select(program_from(ff->program), in.t, ff->keep.data(), (int)ff->keep.size()));
-        if (!f.t) { b2_handle fh = 0; int rc = b2_filter(ff->program, to_handle(in.t), &fh); if (rc != B2_OK) throw Error(rc, b2_last_error()); f = TableRef(from_handle_owned(fh)); }
-        ff->num_output_rows += f.t->rows; ff->num_output_batches++;
-        in = std::move(f);
+        in = TableRef(ff->apply(in.t));
+        ff->count(in.t->rows);
       }
       std::vector<int32_t> offs(world + 1, 0);
       TableRef part;
@@ -1695,19 +1656,14 @@ struct GpuShuffleExchangeExec : GpuExec {
           for (int r = 1; r <= world; r++) offs[r] = (int32_t)in.t->rows;
         } else {
           b2_handle ph = 0;
-          int rc = b2_hash_partition(to_handle(in.t), key_cols.data(), (int)key_cols.size(), 42, world, &ph, offs.data());
-          if (rc != B2_OK) throw Error(rc, b2_last_error());
+          ok(b2_hash_partition(to_handle(in.t), key_cols.data(), (int)key_cols.size(), 42, world, &ph, offs.data()));
           part = TableRef(from_handle_owned(ph));
         }
       }
-      int rc = b2_exchange_ex(comm, part.t ? to_handle(part.t) : 0, part.t ? offs.data() : nullptr, &out, &any);
-      if (rc != B2_OK) throw Error(rc, b2_last_error());
+      ok(b2_exchange_ex(comm, part.t ? to_handle(part.t) : 0, part.t ? offs.data() : nullptr, &out, &any));
     }
     int32_t any_more = 1;
-    {
-      int rc = b2_comm_any_more(comm, &any_more);
-      if (rc != B2_OK) throw Error(rc, b2_last_error());
-    }
+    ok(b2_comm_any_more(comm, &any_more));
     if (!any_more) finished = true;            // every rank sent its last batch (or had none): no further round
     if (!any) { finished = true; if (out) table_release(from_handle_owned(out)); return nullptr; }
     return from_handle_owned(out);
@@ -1728,23 +1684,16 @@ struct GpuBroadcastExchangeExec : GpuExec {
   Table* do_next() override {
     if (done) return nullptr;
     done = true;
-    std::vector<TableRef> parts;
-    while (true) { TableRef b(children[0]->next()); if (!b.t) break; parts.emplace_back(b.release()); }
-    TableRef mine;
-    if (parts.size() == 1) mine = std::move(parts[0]);
-    else if (parts.size() > 1) { std::vector<const Table*> ts; for (auto& p : parts) ts.push_back(p.t); mine = TableRef(concat_tables(ts)); }
+    TableRef mine(one_table(pull_all(children[0])));
     if (world == 1 || !comm) return mine.release();
     if (!mine.t) throw Error(B2_ERR_UNSUPPORTED, "broadcast of a slice with no batches needs the schema (push an empty batch)");
     std::vector<TableRef> got;
     for (int r = 0; r < world; r++) {
       b2_handle out = 0;
-      int rc = b2_broadcast_table(comm, r == rank ? to_handle(mine.t) : 0, r, &out);
-      if (rc != B2_OK) throw Error(rc, b2_last_error());
+      ok(b2_broadcast_table(comm, r == rank ? to_handle(mine.t) : 0, r, &out));
       got.emplace_back(from_handle_owned(out));
     }
-    std::vector<const Table*> ts;
-    for (auto& g : got) ts.push_back(g.t);
-    return concat_tables(ts);
+    return one_table(std::move(got));
   }
 };
 

@@ -258,41 +258,6 @@ __global__ void __launch_bounds__(256) join_probe_distinct_kernel(const __grid_c
   }
 }
 
-// Keeps a region (the Bloom filter) in the persisting part of L2 while probe kernels stream the probe columns past it
-// (cudaStreamAttributeAccessPolicyWindow); off unless B2_JOIN_BLOOM_PERSIST is set.
-struct L2Persist {
-  bool on = false;
-  L2Persist(void* p, size_t bytes) {
-    static const bool enabled = getenv("B2_JOIN_BLOOM_PERSIST") != nullptr;
-    if (!enabled || !p || !bytes) return;
-    static size_t max_window = 0, carve = 0;
-    static bool init = false;
-    if (!init) {
-      init = true;
-      int dev = 0; cudaGetDevice(&dev);
-      cudaDeviceProp prop; cudaGetDeviceProperties(&prop, dev);
-      carve = std::min<size_t>((size_t)prop.persistingL2CacheMaxSize, (size_t)48 << 20);
-      max_window = (size_t)prop.accessPolicyMaxWindowSize;
-      if (carve) cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, carve);
-    }
-    if (!carve || !max_window) return;
-    cudaStreamAttrValue a; memset(&a, 0, sizeof(a));
-    a.accessPolicyWindow.base_ptr = p;
-    a.accessPolicyWindow.num_bytes = std::min(bytes, max_window);
-    a.accessPolicyWindow.hitRatio = (float)std::min(1.0, (double)carve / (double)a.accessPolicyWindow.num_bytes);
-    a.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
-    a.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-    on = cudaStreamSetAttribute(stream(), cudaStreamAttributeAccessPolicyWindow, &a) == cudaSuccess;
-    if (!on) cudaGetLastError();
-  }
-  ~L2Persist() {
-    if (!on) return;
-    cudaStreamAttrValue a; memset(&a, 0, sizeof(a));
-    a.accessPolicyWindow.num_bytes = 0;
-    cudaStreamSetAttribute(stream(), cudaStreamAttributeAccessPolicyWindow, &a);
-  }
-};
-
 // The commonest probe of all — INNER join against a distinct build side on ONE integer key column without NULLs (every
 // FK -> PK join of TPC-H) — without the generic row machinery (KeyCols loops, validity, runtime join kind): ~6x fewer
 // instructions per row than join_probe_distinct_kernel.  A warp takes PQ x 32 rows at a time (probe_distinct1_rows):
@@ -748,6 +713,27 @@ static JoinTracker* tracker_from(b2_handle h) {
   return reinterpret_cast<JoinTracker*>((intptr_t)h);
 }
 
+// the instances of the one-key probes, by key type K: (SEL, TRACK, DIRECT) of join_probe_distinct1_kernel, (TRACK, DIRECT) of
+// join_filter_probe_kernel and, with EMIT, its direct choice (the emitting probe does not track)
+template <typename K>
+static auto distinct1_instance(bool sel, bool track, bool direct) {
+  decltype(&join_probe_distinct1_kernel<K, false, false>) const k[8] = {
+      join_probe_distinct1_kernel<K, false, false, false>, join_probe_distinct1_kernel<K, false, false, true>,
+      join_probe_distinct1_kernel<K, false, true, false>,  join_probe_distinct1_kernel<K, false, true, true>,
+      join_probe_distinct1_kernel<K, true, false, false>,  join_probe_distinct1_kernel<K, true, false, true>,
+      join_probe_distinct1_kernel<K, true, true, false>,   join_probe_distinct1_kernel<K, true, true, true>};
+  return k[4 * sel + 2 * track + direct];
+}
+template <typename K, bool EMIT>
+static auto filter_probe_instance(bool track, bool direct) {
+  if constexpr (EMIT) return direct ? join_filter_probe_kernel<K, false, true, true> : join_filter_probe_kernel<K, false, true, false>;
+  else {
+    decltype(&join_filter_probe_kernel<K, false>) const k[4] = {join_filter_probe_kernel<K, false, false, false>, join_filter_probe_kernel<K, false, false, true>,
+                                                                join_filter_probe_kernel<K, true, false, false>, join_filter_probe_kernel<K, true, false, true>};
+    return k[2 * track + direct];
+  }
+}
+
 // GpuFilter directly below the stream side of an INNER FK -> PK join, fused INTO the probe (join_filter_probe_kernel) when
 // the predicate is of the simple shape (simplefilter.cuh) and the probe qualifies for the one-key distinct probe: the gather
 // maps carry ORIGINAL row ids of `batch`, `npass_out` = rows that passed the filter (the filter node's numOutputRows).
@@ -766,6 +752,33 @@ static bool filter_probe_applies(const JoinTable* jt, const Table* batch, int ke
   return simple_pred_of(prog, batch, sp);   // also: every predicate column 16-byte aligned
 }
 
+// join_filter_probe_kernel over the n rows of a batch whose key column is pc and predicate sp: the gather maps into lp / rp (the
+// build rows found marked in `track` when given) or, given `em`, the output rows.  h = {matches, rows that passed the filter}
+static void filter_probe(const JoinTable* jt, const Column* pc, const SimplePred& sp, int64_t n, int32_t* lp, int32_t* rp, uint32_t* track,
+                         const EmitCols* em, unsigned long long h[2]) {
+  DevBuf tot(16);
+  CUDA_CHECK(cudaMemsetAsync(tot.p, 0, 16, stream()));
+  const HashView hv = hash_view(jt);
+  const DirectMap dm = direct_map(jt);
+  unsigned long long* tp = tot.as<unsigned long long>();
+  auto run = [&](auto* keys, auto emit) {
+    typedef std::remove_const_t<std::remove_pointer_t<decltype(keys)>> K;
+    constexpr bool EMIT = decltype(emit)::value;
+    typename std::conditional<EMIT, EmitCols, NoEmit>::type e;
+    if constexpr (EMIT) e = *em;
+    launch(track ? "join_filter_probe_track_kernel" : "join_filter_probe_kernel", filter_probe_instance<K, EMIT>(track != nullptr, jt->direct),
+           grid_for(n, FP_TILE, FP_CTAS), SF_NT, 0, stream(), sp, keys, n, hv.slots, hv.mask, hv.bloom, hv.bloom_mask, tp, lp, rp, tp + 1, track, e, dm);
+  };
+  auto by_key = [&](auto emit) {
+    if (dtype_width(pc->dtype) == 8) run(pc->data.as<int64_t>(), emit);
+    else run(pc->data.as<int32_t>(), emit);
+  };
+  if (em) by_key(std::true_type());
+  else by_key(std::false_type());
+  d2h(h, tot.p, 2);
+  sync();
+}
+
 bool join_probe_pred(b2_handle ht, const Table* batch, int key_col, const Program* prog, Column** out_lm, Column** out_rm, int64_t* npass_out,
                      b2_handle tracker) {
   JoinTable* jt = jt_from(ht);
@@ -779,36 +792,9 @@ bool join_probe_pred(b2_handle ht, const Table* batch, int key_col, const Progra
   const Column* pc = nullptr;
   SimplePred sp;
   if (!filter_probe_applies(jt, batch, key_col, prog, pc, sp)) return false;
-  const int pw = dtype_width(pc->dtype);
   ColGuard lm(new_column(B2_INT32, 0, n, false)), rm(new_column(B2_INT32, 0, n, false));
-  DevBuf tot(16);
-  CUDA_CHECK(cudaMemsetAsync(tot.p, 0, 16, stream()));
-  {
-    const int grid = grid_for(n, FP_TILE, FP_CTAS);
-    const HashView hv = hash_view(jt);
-    const uint64_t* sl = hv.slots; const uint32_t msk = hv.mask;
-    const unsigned long long* bl = hv.bloom;
-    unsigned long long* tp = tot.as<unsigned long long>();
-    int32_t* lp = lm.c->data.as<int32_t>(); int32_t* rp = rm.c->data.as<int32_t>();
-    const NoEmit ne;
-    const DirectMap dm = direct_map(jt);
-    const bool d = jt->direct;
-    if (track) {
-      if (pw == 8) launch("join_filter_probe_track_kernel", d ? join_filter_probe_kernel<int64_t, true, false, true> : join_filter_probe_kernel<int64_t, true>,
-                          grid, SF_NT, 0, stream(), sp, pc->data.as<int64_t>(), n, sl, msk, bl, hv.bloom_mask, tp, lp, rp, tp + 1, track, ne, dm);
-      else launch("join_filter_probe_track_kernel", d ? join_filter_probe_kernel<int32_t, true, false, true> : join_filter_probe_kernel<int32_t, true>,
-                  grid, SF_NT, 0, stream(), sp, pc->data.as<int32_t>(), n, sl, msk, bl, hv.bloom_mask, tp, lp, rp, tp + 1, track, ne, dm);
-    } else if (pw == 8) {
-      launch("join_filter_probe_kernel", d ? join_filter_probe_kernel<int64_t, false, false, true> : join_filter_probe_kernel<int64_t, false>, grid, SF_NT, 0,
-             stream(), sp, pc->data.as<int64_t>(), n, sl, msk, bl, hv.bloom_mask, tp, lp, rp, tp + 1, nullptr, ne, dm);
-    } else {
-      launch("join_filter_probe_kernel", d ? join_filter_probe_kernel<int32_t, false, false, true> : join_filter_probe_kernel<int32_t, false>, grid, SF_NT, 0,
-             stream(), sp, pc->data.as<int32_t>(), n, sl, msk, bl, hv.bloom_mask, tp, lp, rp, tp + 1, nullptr, ne, dm);
-    }
-  }
   unsigned long long h[2] = {0, 0};
-  d2h(h, tot.p, 2);
-  sync();
+  filter_probe(jt, pc, sp, n, lm.c->data.as<int32_t>(), rm.c->data.as<int32_t>(), track, nullptr, h);
   lm.c->size = (int64_t)h[0]; rm.c->size = (int64_t)h[0];
   *npass_out = (int64_t)h[1];
   *out_lm = lm.release(); *out_rm = rm.release();
@@ -903,27 +889,8 @@ bool join_probe_pred_emit(b2_handle ht, const Table* batch, int key_col, const P
     em.b_out[em.nb++] = outs.v.back()->data.p;
   }
   em.pw = pl.width; em.packed = pl.packed.p; em.cap = (unsigned long long)cap;
-  const int64_t n = batch->rows;
-  DevBuf tot(16);
-  CUDA_CHECK(cudaMemsetAsync(tot.p, 0, 16, stream()));
-  {
-    const int grid = grid_for(n, FP_TILE, FP_CTAS);
-    const HashView hv = hash_view(jt);
-    const uint64_t* sl = hv.slots; const uint32_t msk = hv.mask;
-    const unsigned long long* bl = hv.bloom;
-    unsigned long long* tp = tot.as<unsigned long long>();
-    const DirectMap dm = direct_map(jt);
-    const bool d = jt->direct;
-    if (dtype_width(pc->dtype) == 8)
-      launch("join_filter_probe_kernel", d ? join_filter_probe_kernel<int64_t, false, true, true> : join_filter_probe_kernel<int64_t, false, true>, grid,
-             SF_NT, 0, stream(), sp, pc->data.as<int64_t>(), n, sl, msk, bl, hv.bloom_mask, tp, nullptr, nullptr, tp + 1, nullptr, em, dm);
-    else
-      launch("join_filter_probe_kernel", d ? join_filter_probe_kernel<int32_t, false, true, true> : join_filter_probe_kernel<int32_t, false, true>, grid,
-             SF_NT, 0, stream(), sp, pc->data.as<int32_t>(), n, sl, msk, bl, hv.bloom_mask, tp, nullptr, nullptr, tp + 1, nullptr, em, dm);
-  }
   unsigned long long h[2] = {0, 0};
-  d2h(h, tot.p, 2);
-  sync();
+  filter_probe(jt, pc, sp, batch->rows, nullptr, nullptr, nullptr, &em, h);
   *total_out = (int64_t)h[0];
   *npass_out = (int64_t)h[1];
   if ((int64_t)h[0] <= cap) {
@@ -1075,7 +1042,7 @@ static bool hash_build(JoinTable* jt) {
     // bits per key: fewer bits = more false positives (each costs one random HBM slot read) but a smaller filter.  SF100 q3
     // step on one H100 SXM (700 W): 8 bits 37.6 ms (probe 8.8), 16 bits 40.6 ms (probe 11.3): the 32 MB filter of the
     // 14.6 M-row build side crowds the 50 MB L2, the 16 MB one does not.  Pinning the 16-bit filter in the persisting part
-    // of L2 (B2_JOIN_BLOOM_PERSIST) was slower still (55.5 ms)
+    // of L2 was slower still (55.5 ms)
     static const int bits_per_key = getenv("B2_JOIN_BLOOM_BITS") ? std::max(2, atoi(getenv("B2_JOIN_BLOOM_BITS"))) : 8;
     int64_t words = 1 << 15;
     while (words * 64 < t->rows * bits_per_key && words < (4 << 20)) words <<= 1;   // at most 32 MB
@@ -1202,37 +1169,17 @@ static void probe_maps(JoinTable* jt, Table* pt, b2_handle selection, int32_t ki
     if (n) {
       DevBuf tot(8);
       CUDA_CHECK(cudaMemsetAsync(tot.p, 0, 8, stream()));
-      L2Persist keep(jt->direct && one_key ? nullptr : jt->bloom.p, jt->direct && one_key ? 0 : jt->bloom.bytes);
       if (one_key) {
-        const int grid = grid_for(n, 256);
         const HashView hv = hash_view(jt);
-        const uint64_t* sl = hv.slots; const uint32_t msk = hv.mask;
-        const unsigned long long* bl = hv.bloom; unsigned long long* tp = tot.as<unsigned long long>();
-        int32_t* lp = lm.c->data.as<int32_t>(); int32_t* rp = rm.c->data.as<int32_t>();
         const DirectMap dm = direct_map(jt);
-        const bool d = jt->direct;
-        if (track) {
-          if (pw == 8)
-            launch("join_probe_distinct1_track_kernel",
-                   d ? (sel ? join_probe_distinct1_kernel<int64_t, true, true, true> : join_probe_distinct1_kernel<int64_t, false, true, true>)
-                     : (sel ? join_probe_distinct1_kernel<int64_t, true, true> : join_probe_distinct1_kernel<int64_t, false, true>),
-                   grid, 256, 0, stream(), pc->data.as<int64_t>(), sel, n, sl, msk, bl, hv.bloom_mask, tp, lp, rp, track, dm);
-          else
-            launch("join_probe_distinct1_track_kernel",
-                   d ? (sel ? join_probe_distinct1_kernel<int32_t, true, true, true> : join_probe_distinct1_kernel<int32_t, false, true, true>)
-                     : (sel ? join_probe_distinct1_kernel<int32_t, true, true> : join_probe_distinct1_kernel<int32_t, false, true>),
-                   grid, 256, 0, stream(), pc->data.as<int32_t>(), sel, n, sl, msk, bl, hv.bloom_mask, tp, lp, rp, track, dm);
-        } else if (pw == 8) {
-          launch("join_probe_distinct1_kernel",
-                 d ? (sel ? join_probe_distinct1_kernel<int64_t, true, false, true> : join_probe_distinct1_kernel<int64_t, false, false, true>)
-                   : (sel ? join_probe_distinct1_kernel<int64_t, true, false> : join_probe_distinct1_kernel<int64_t, false, false>),
-                 grid, 256, 0, stream(), pc->data.as<int64_t>(), sel, n, sl, msk, bl, hv.bloom_mask, tp, lp, rp, nullptr, dm);
-        } else {
-          launch("join_probe_distinct1_kernel",
-                 d ? (sel ? join_probe_distinct1_kernel<int32_t, true, false, true> : join_probe_distinct1_kernel<int32_t, false, false, true>)
-                   : (sel ? join_probe_distinct1_kernel<int32_t, true, false> : join_probe_distinct1_kernel<int32_t, false, false>),
-                 grid, 256, 0, stream(), pc->data.as<int32_t>(), sel, n, sl, msk, bl, hv.bloom_mask, tp, lp, rp, nullptr, dm);
-        }
+        auto probe1 = [&](auto* keys) {
+          typedef std::remove_const_t<std::remove_pointer_t<decltype(keys)>> K;
+          launch(track ? "join_probe_distinct1_track_kernel" : "join_probe_distinct1_kernel", distinct1_instance<K>(sel != nullptr, track != nullptr, jt->direct),
+                 grid_for(n, 256), 256, 0, stream(), keys, sel, n, hv.slots, hv.mask, hv.bloom, hv.bloom_mask, tot.as<unsigned long long>(),
+                 lm.c->data.as<int32_t>(), rm.c->data.as<int32_t>(), track, dm);
+        };
+        if (pw == 8) probe1(pc->data.as<int64_t>());
+        else probe1(pc->data.as<int32_t>());
       } else {
         launch(track ? "join_probe_distinct_track_kernel" : "join_probe_distinct_kernel",
                track ? join_probe_distinct_kernel<true> : join_probe_distinct_kernel<false>, grid_for(n, 256), 256, 0, stream(), pk, bk, n,
