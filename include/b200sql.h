@@ -306,7 +306,9 @@ int b2_top_n(b2_handle table, const b2_order_by_arg* keys, int32_t nkeys, int64_
              b2_handle* out_table);                                    /* GpuTopN */
 int b2_merge_sorted(const b2_handle* tables, int32_t ntables, const b2_order_by_arg* keys,
                     int32_t nkeys, b2_handle* out_table);              /* Table.merge */
-/* Table.lowerBound / upperBound: for each row of `values`, its insertion index in sorted `table` */
+/* Table.lowerBound / upperBound: for each row of `values`, its insertion index in sorted `table`.  Both tables hold the key
+ * columns, in key order.  B2_ERR_INVALID: key dtypes or decimal scales differ; B2_ERR_UNSUPPORTED: a STRING key.
+ * b2_merge_sorted, like b2_concat: B2_ERR_INVALID when a column's dtype or decimal scale differs between tables. */
 int b2_search_bounds(b2_handle sorted_table, b2_handle values_table, const b2_order_by_arg* keys,
                      int32_t nkeys, int32_t upper, b2_handle* out_int32_idx);
 /* GpuSortExec with the out-of-core sort (GpuSortExec.scala:130-165, GpuOutOfCoreSortIterator :241-630): a stable full sort

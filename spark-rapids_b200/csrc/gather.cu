@@ -173,6 +173,7 @@ Table* concat_tables(const std::vector<const Table*>& ts) {
     bool any_null = false;
     for (auto* t : ts) {
       B2_CHECK(t->cols[c]->dtype == c0->dtype, "concat: dtype differs");
+      B2_CHECK(!is_decimal(c0->dtype) || t->cols[c]->scale == c0->scale, "concat: decimal scale differs");
       any_null = any_null || t->cols[c]->nullable();
     }
     if (c0->dtype == B2_STRING) {

@@ -297,7 +297,7 @@ int64_t lower_bound_row(const Table* sorted, const Table* probe, const b2_order_
   B2_CHECK(probe->rows >= 1, "bounds: empty probe");
   std::vector<SortPlan> p = shared_sort_plans({sorted, probe}, keys, nkeys);
   DevBuf out(4);
-  launch(bounds_kernel, 1, 32, 0, stream(), p[0], p[1], sorted->rows, 1, 0, out.as<int32_t>());
+  launch("bounds_kernel", bounds_kernel, 1, 32, 0, stream(), p[0], p[1], sorted->rows, 1, 0, out.as<int32_t>());
   int32_t h = 0;
   d2h(&h, out.p, 1);
   sync();
@@ -493,7 +493,7 @@ static Table* top_n_select(const Table* t, const b2_order_by_arg* keys, int nkey
   for (int chunk = 0; chunk < nchunks && m < 0; chunk++) {
     launch(build_chunk_kernel, grid_for(n, 256), 256, 0, stream(), plan, nullptr, n, chunk, k0.as<uint64_t>());
     CUDA_CHECK(cudaMemsetAsync(hist.p, 0, hist.bytes, stream()));
-    launch(hist8_kernel, grid_for(n, 256 * 8), 256, 0, stream(), k0.as<uint64_t>(), n, 8, hist.as<unsigned long long>());
+    launch("topn_hist8_kernel", hist8_kernel, grid_for(n, 256 * 8), 256, 0, stream(), k0.as<uint64_t>(), n, 8, hist.as<unsigned long long>());
     std::vector<unsigned long long> h(8 * 256);
     d2h(h.data(), hist.p, h.size());
     sync();
@@ -521,14 +521,14 @@ static Table* top_n_select(const Table* t, const b2_order_by_arg* keys, int nkey
       if (d == 0 || tied <= 8192) { thr = pval | (d > 0 ? (1ull << (8 * d)) - 1 : 0); m = below + tied; break; }
       d--;
       CUDA_CHECK(cudaMemsetAsync(hist.p, 0, 256 * 8, stream()));
-      launch(hist_prefix_kernel, grid_for(n, 256 * 8), 256, 0, stream(), k0.as<uint64_t>(), n, pmask, pval, 8 * d, hist.as<unsigned long long>());
+      launch("hist_prefix_kernel", hist_prefix_kernel, grid_for(n, 256 * 8), 256, 0, stream(), k0.as<uint64_t>(), n, pmask, pval, 8 * d, hist.as<unsigned long long>());
       d2h(hd.data(), hist.p, 256);
       sync();
     }
   }
   if (m < 0 || m > n / 4) return nullptr;   // all leading bytes equal, or one value dominates: sort everything
   ColGuard mask(new_column(B2_BOOL8, 0, n, false));
-  launch(topn_mask_kernel, grid_for(n, 256), 256, 0, stream(), k0.as<uint64_t>(), n, thr, mask.c->data.as<int8_t>());
+  launch("topn_mask_kernel", topn_mask_kernel, grid_for(n, 256), 256, 0, stream(), k0.as<uint64_t>(), n, thr, mask.c->data.as<int8_t>());
   std::unique_ptr<Table, void (*)(Table*)> sub(filter_by_mask(t, mask.c), table_release);
   if (sub->rows < std::min<int64_t>(limit, n)) throw Error(B2_ERR_INVALID, "top-n selection lost rows");
   DevBuf perm = sort_order(sub.get(), keys, nkeys);
@@ -600,11 +600,13 @@ int b2_search_bounds(b2_handle sorted_table, b2_handle values_table, const b2_or
   B2_CHECK((int)st->cols.size() >= nkeys && (int)vt->cols.size() >= nkeys, "bounds tables must hold the key columns");
   for (int i = 0; i < nkeys; i++) {
     B2_CHECK(st->cols[i]->dtype == vt->cols[i]->dtype, "bounds: key dtypes differ");
+    // the normalised key compares unscaled integers: 1.00 (100 at scale 2) and 1.0000 (10000 at scale 4) would differ
+    B2_CHECK(!is_decimal(st->cols[i]->dtype) || st->cols[i]->scale == vt->cols[i]->scale, "bounds: decimal key scales differ");
     if (st->cols[i]->dtype == B2_STRING) throw Error(B2_ERR_UNSUPPORTED, "bounds search over string keys");
   }
   SortPlan sp = make_sort_plan(st, k.data(), nkeys, true), vp = make_sort_plan(vt, k.data(), nkeys, true);
   ColGuard out(new_column(B2_INT32, 0, vt->rows, false));
-  if (vt->rows) launch(bounds_kernel, grid_for(vt->rows, 128), 128, 0, stream(), sp, vp, st->rows, vt->rows, upper, out.c->data.as<int32_t>());
+  if (vt->rows) launch("bounds_kernel", bounds_kernel, grid_for(vt->rows, 128), 128, 0, stream(), sp, vp, st->rows, vt->rows, upper, out.c->data.as<int32_t>());
   *out_int32_idx = to_handle(out.release());
   B2_CATCH
 }
