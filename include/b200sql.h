@@ -529,10 +529,10 @@ int b2_exec_hash_aggregate(b2_handle child, b2_handle program, int32_t has_predi
 int b2_exec_aggregate_set_repartitioning(b2_handle agg, int64_t target_bytes, int32_t num_buckets);
 /* out4: first-level buckets (0 = never bucketed), buckets split again, bytes split over all levels, deepest level reached */
 int b2_exec_aggregate_repartition_stats(b2_handle agg, int64_t* out4);
-/* GpuShuffledHashJoinExec (GpuShuffledHashJoinExec.scala:228-385): output = stream columns ++ build columns.  RIGHT_OUTER joins
- * the stream batches one at a time, tracking the build rows found (b2_join_probe_track), and after the last one emits the
- * unmatched build rows with NULL stream columns, in batches halved until they fit; no stream batch at all, or no build
- * batch: B2_ERR_UNSUPPORTED.  FULL_OUTER without a condition coalesces the stream side into one batch. */
+/* GpuShuffledHashJoinExec (GpuShuffledHashJoinExec.scala:228-385): output = stream columns ++ build columns.  RIGHT_OUTER
+ * and FULL_OUTER join the stream batches one at a time (as INNER and LEFT_OUTER), tracking the build rows found
+ * (b2_join_probe_track), and after the last one emit the unmatched build rows with NULL stream columns, in batches halved
+ * until they fit; no stream batch at all, or no build batch: B2_ERR_UNSUPPORTED. */
 int b2_exec_shuffled_hash_join(b2_handle stream_child, b2_handle build_child, const int32_t* stream_keys,
                                const int32_t* build_keys, int32_t nkeys, int32_t kind, int32_t nulls_equal, b2_handle* out);
 /* same with a column-pruning GpuProjectExec above the join fused into the gathers: output = stream_out ++ build_out */
@@ -548,9 +548,8 @@ int b2_exec_join_set_condition(b2_handle join, b2_handle condition_program);
 /* GpuSubPartitionHashJoin (GpuShuffledHashJoinExec.scala:228-281, GpuSubPartitionHashJoin.scala:86-617): when the build side
  * passes target_bytes (table_bytes; raised to 16 KiB) both sides are split into num_partitions (2..256; Spark default 16,
  * RapidsConf.scala:2660) spillable buckets by murmur3 seed 100 of the join keys and joined bucket by bucket; adjacent small
- * buckets are packed up to the target, a bucket still over it (FULL OUTER without a condition: by its build or its stream
- * side) is split once
- * more (seed 110) and then joined as it is, so the rows of a single key must fit on the device.  Without this call, or when the build side stays within target_bytes,
+ * buckets are packed up to the target, a bucket still over it is split once more (seed 110) and then joined as it is, so
+ * the rows of a single key must fit on the device.  Without this call, or when the build side stays within target_bytes,
  * the join is unchanged. */
 int b2_exec_join_set_sub_partitioning(b2_handle join, int64_t target_bytes, int32_t num_partitions);
 /* out4: first-level buckets (0 = not sub-partitioned), buckets repartitioned, build bytes split, stream bytes split */

@@ -5,12 +5,14 @@ no o_comment, so the predicate is o_orderdate < 1997-01-01 (about 70 % of the or
   (a) today's plan: LEFT OUTER, stream customer, build the filtered orders (a non-distinct build side: the generic probe);
   (b) RIGHT OUTER (= LeftOuter / BuildLeft with the children swapped): build customer, stream orders, the filter fused into
       the probe (join_filter_probe_track_kernel), the unmatched customers emitted at the end (tracker_count / tracker_write);
-  (c) the probe of (b) as INNER against RIGHT OUTER: the cost of tracking.
+  (c) the probe of (b) as INNER against RIGHT OUTER: the cost of tracking;
+  (d) (b) as FULL OUTER without a condition: the filtered orders probe LEFT OUTER, tracked, one stream batch at a time.
 
 Every arm runs the GpuShuffledHashJoinExec over device-resident batches (8 chunks per table).  Reported per arm: wall ms
 (host clock around the whole join and a device synchronise, profiler off, the arms alternated, median of --reps), per-kernel
 ms from a separate profiled call, the bytes the probe and tracker kernels need (below) over their kernel time against the
-3.35 TB/s H100 SXM data sheet, and count(*) per c_custkey, checked equal between (a) and (b).  The card and its power limit
+3.35 TB/s H100 SXM data sheet, and count(*) per c_custkey, checked equal between (a) and (b) and, for the rows of (d) that
+carry a customer, between (b) and (d); (d) also reports its output rows.  The card and its power limit
 are read in the same run.  One JSON line per measurement.
   filter probe:     4 B o_orderdate per order, 8 B o_custkey + one 16-byte table slot per passing order, 8 B of maps per pair
   tracker kernels:  nb / 8 bytes of bitmap read twice, 4 B per unmatched customer written
@@ -66,7 +68,7 @@ def main():
         filtered = E.GpuFilterExec(pred, E.GpuBatchSource(orders))
         if arm == "a":   # stream customer, build the filtered orders; out: c_custkey, o_orderkey
             return E.GpuShuffledHashJoinExec([0], [1], m.JOIN_LEFT_OUTER, E.GpuBatchSource(cust), filtered, stream_out=[0], build_out=[0])
-        kind = m.JOIN_RIGHT_OUTER if arm == "b" else m.JOIN_INNER   # stream the filtered orders, build customer; out: o_orderkey, c_custkey
+        kind = {"b": m.JOIN_RIGHT_OUTER, "c": m.JOIN_INNER, "d": m.JOIN_FULL_OUTER}[arm]   # stream the filtered orders, build customer; out: o_orderkey, c_custkey
         return E.GpuShuffledHashJoinExec([1], [0], kind, filtered, E.GpuBatchSource(cust), stream_out=[0], build_out=[0])
 
     def run(arm, keep=False):
@@ -78,14 +80,18 @@ def main():
             return None
         return outs
 
-    def counts(arm, outs):
+    def counts(arm, outs, without_customer=None):
         ck, ok = (0, 1) if arm == "a" else (1, 0)
         cnt = np.zeros(ncust, np.int64)
         rows = np.zeros(ncust, np.int64)
         for t in outs:
             c, cv = t.column(ck).to_numpy()
             _, ov = t.column(ok).to_numpy()
-            assert cv.all()
+            if without_customer is None:
+                assert cv.all()
+            else:   # FULL OUTER: orders without a customer keep a NULL c_custkey
+                without_customer.append(int((~cv).sum()))
+                c, ov = c[cv], ov[cv]
             np.add.at(rows, c, 1)
             np.add.at(cnt, c[ov], 1)
         return cnt, rows
@@ -96,22 +102,29 @@ def main():
     assert np.array_equal(ca, cb), "count per c_custkey differs between (a) and (b)"
     assert (rb >= 1).all() and (ra >= 1).all()
     unmatched = int((cb == 0).sum())
-    print(json.dumps({"check": "count(*) per c_custkey equal in (a) and (b)", "sf": args.sf, "customers": ncust, "orders": nord,
-                      "orders_passing": int(cb.sum()), "customers_without_orders": unmatched}), flush=True)
+    outs_d = run("d", True)
+    nd = []
+    cd, rd = counts("d", outs_d, nd)
+    assert np.array_equal(cd, cb) and np.array_equal(rd, rb), "count per c_custkey differs between (b) and (d)"
+    print(json.dumps({"check": "count(*) per c_custkey equal in (a) and (b), and in (b) and (d)", "sf": args.sf, "customers": ncust,
+                      "orders": nord, "orders_passing": int(cb.sum()), "customers_without_orders": unmatched,
+                      "full_outer_rows": sum(t.num_rows for t in outs_d), "full_outer_batches": len(outs_d),
+                      "full_outer_rows_without_customer": sum(nd)}), flush=True)
+    del outs_d
     gc.collect()
 
     # wall: arms alternated, profiler off
-    walls = {a: [] for a in "abc"}
-    for a in "abc":
+    walls = {a: [] for a in "abcd"}
+    for a in "abcd":
         run(a)   # warm-up
     for _ in range(args.reps):
-        for a in "abc":
+        for a in "abcd":
             m.sync()
             t0 = time.perf_counter()
             run(a)
             walls[a].append((time.perf_counter() - t0) * 1e3)
     # per-kernel ms, one profiled call per arm
-    for a in "abc":
+    for a in "abcd":
         m.profile_enable(True)
         try:
             run(a)
@@ -120,7 +133,7 @@ def main():
             m.profile_enable(False)
         npass = int(cb.sum())
         rec = {"arm": {"a": "left outer, build filtered orders", "b": "right outer, build customer, filter in probe",
-                       "c": "inner, build customer, filter in probe"}[a],
+                       "c": "inner, build customer, filter in probe", "d": "full outer, build customer, no condition"}[a],
                "sf": args.sf, "wall_ms": [round(x, 2) for x in walls[a]], "wall_ms_median": round(float(np.median(walls[a])), 2),
                "kernel_ms": kern, "gpu": info.get("name"), "power_limit": info.get("power.limit"), "sm_clock_max": info.get("clocks.max.sm")}
         probe_k = "join_filter_probe_track_kernel" if a == "b" else "join_filter_probe_kernel"

@@ -11,7 +11,7 @@
 //   GpuHashAggregateExec      GpuAggregateExec.scala:1942-2085; first pass per batch (:730-742) then
 //                             GpuMergeAggregateIterator (:896-1018): concat partials + merge-aggregate
 //   GpuShuffledHashJoinExec   GpuShuffledHashJoinExec.scala:228-385 + GpuHashJoin.doJoin (:2547-2628):
-//                             build side coalesced to ONE batch, hash table built once, stream probed
+//                             build side concatenated into ONE batch, hash table built once, stream probed
 //                             batch by batch, payload gathered
 //   GpuSortExec / GpuTopN     GpuSortExec.scala:87-165 (each-batch | full), limit.scala:234-330
 //   GpuCoalesceBatches        GpuCoalesceBatches.scala:160-239 (TargetSize goal by rows)
@@ -647,7 +647,7 @@ struct GpuHashAggregateExec : GpuExec {
 struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), children[1] = build (right)
   std::vector<int> stream_keys, build_keys;
   int kind = B2_JOIN_INNER;
-  bool nulls_equal = false, built = false, full_done = false;
+  bool nulls_equal = false, built = false;
   // mixed join (GpuHashJoin.scala:335-530 mixed*JoinGatherMaps, :1556 ConditionalHashJoinIterator): an extra non-equi
   // condition, bound over [stream columns ++ build columns], decides which equi-matched pairs survive
   b2_handle condition = 0;
@@ -655,10 +655,10 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
   std::vector<int> stream_out, build_out;    // pruned: the columns each side contributes (in this order)
   TableRef build_table;
   b2_handle ht = 0;
-  // Outer joins that preserve the build side — RIGHT OUTER, and FULL OUTER with a condition — are "tracked" (HashOuterJoinIterator,
-  // GpuHashJoin.scala:1807-1814): stream batches are joined one at a time (INNER / the conditional LEFT OUTER), a tracker over
-  // the hash table keeps the build rows that found a partner, and once the stream side is exhausted the others come out
-  // with NULL stream columns (getFinalBatch, :2288-2326).  FULL OUTER without a condition coalesces its stream side instead.
+  // Outer joins that preserve the build side — RIGHT OUTER and FULL OUTER — are "tracked" (HashOuterJoinIterator,
+  // GpuHashJoin.scala:1807-1814): stream batches are joined one at a time (INNER / LEFT OUTER, with or without a condition), a
+  // tracker over the hash table keeps the build rows that found a partner, and once the stream side is exhausted the others
+  // come out with NULL stream columns (getFinalBatch, :2288-2326).
   b2_handle tracker = 0;
   // zero rows of the stream side as the join sees it, which stream_out indexes (the filter's output when one is fused, the carried
   // columns when sub-partitioned): the NULL side of the final rows, and the schema of a sub-partition pair without stream rows
@@ -671,8 +671,7 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
     if (tracker) b2_join_tracker_close(tracker);
     if (ht) b2_join_hash_table_close(ht);
   }
-  bool tracked() const { return kind == B2_JOIN_RIGHT_OUTER || (kind == B2_JOIN_FULL_OUTER && condition); }
-  bool coalesced() const { return kind == B2_JOIN_FULL_OUTER && !condition; }
+  bool tracked() const { return kind == B2_JOIN_RIGHT_OUTER || kind == B2_JOIN_FULL_OUTER; }
   // the hash table over build_table's keys and, for a tracked join, its tracker (retry: the build of the table runs under
   // with_retry)
   void build_hash(bool retry) {
@@ -687,11 +686,12 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
     fin_started = false;
     if (tracked()) ok(b2_join_tracker_create(ht, &tracker));
   }
-  // the maps of one stream batch (through a selection vector): RIGHT OUTER probes INNER and marks the build rows it finds
+  // the maps of one stream batch (through a selection vector): a tracked join marks the build rows it finds, probing INNER
+  // for RIGHT OUTER and LEFT OUTER for FULL OUTER
   void probe(const Table* keys, Column* sel, b2_handle* lm, b2_handle* rm) {
-    const b2_handle sh = sel ? to_handle(sel) : 0;
-    ok(kind == B2_JOIN_RIGHT_OUTER ? b2_join_probe_track(ht, to_handle(const_cast<Table*>(keys)), sh, B2_JOIN_INNER, tracker, lm, rm)
-                                   : b2_join_probe_sel(ht, to_handle(const_cast<Table*>(keys)), sh, kind, lm, rm));
+    const b2_handle kh = to_handle(const_cast<Table*>(keys)), sh = sel ? to_handle(sel) : 0;
+    if (!tracked()) { ok(b2_join_probe_sel(ht, kh, sh, kind, lm, rm)); return; }
+    ok(b2_join_probe_track(ht, kh, sh, kind == B2_JOIN_FULL_OUTER ? B2_JOIN_LEFT_OUTER : B2_JOIN_INNER, tracker, lm, rm));
   }
   static Table* select(const Table* t, const std::vector<int>& idx) {
     std::vector<Column*> cols;
@@ -717,7 +717,7 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
   // batch — the filtered copy of the stream side (TPC-H q3: 7.8 GB per pass over lineitem) is never written or re-read.
   GpuFilterExec* fused = nullptr;
   GpuFilterExec* fusable_filter() const {
-    if (kind == B2_JOIN_FULL_OUTER || condition || getenv("B2_NO_FILTER_FUSION")) return nullptr;
+    if (condition || getenv("B2_NO_FILTER_FUSION")) return nullptr;
     return dynamic_cast<GpuFilterExec*>(children[0]);
   }
   // fused: the filter's input columns of the stream keys, of the stream columns joined and of every filter output
@@ -815,17 +815,7 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
       if (Table* t = fused_next()) return t;
       return tracked() ? final_start() : nullptr;
     }
-    TableRef s;
-    if (coalesced()) {
-      // the unmatched build rows can only be emitted once every stream row has been seen: without a condition the stream
-      // side is coalesced into one batch (tracked joins keep the matched build rows across batches instead: final_start)
-      if (full_done) return nullptr;
-      full_done = true;
-      s = TableRef(one_table(pull_all(children[0])));
-      if (!s.t) throw Error(B2_ERR_UNSUPPORTED, "empty stream side of a full outer join needs the stream schema");
-    } else {
-      s = TableRef(children[0]->next());
-    }
+    TableRef s(children[0]->next());
     if (!s.t) return tracked() ? final_start() : nullptr;
     if (tracked() && !stream_schema.t) stream_schema = TableRef(slice_table(s.t, 0, 0));
     todo.emplace_back(std::move(s), 0);
@@ -883,7 +873,7 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
         em_stats[1]++;
         return out;
       } catch (const Error& e) {
-        if (!splittable(e) || st.t->rows < 2 || depth >= 16 || coalesced()) throw;
+        if (!splittable(e) || st.t->rows < 2 || depth >= 16) throw;
         note_split();
         const int64_t mid = st.t->rows / 2;
         // the halves replace the batch: the batch itself is released before they are made, so the split needs no extra room
@@ -898,7 +888,7 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
   // the output rows of stream batch `st` (its columns `scols`; null: all) from the gather maps: stream columns ++ build columns
   // (GpuHashJoin.scala:2451-2470).  Without a right map (semi / anti) or anything wanted from the build side: the stream columns.
   Table* joined_rows(const Table* st, const Column* lmap, const Column* rmap, const std::vector<int>* scols) {
-    TableRef left(gather_table(st, lmap->data.as<int32_t>(), lmap->size, kind == B2_JOIN_FULL_OUTER, scols));
+    TableRef left(gather_table(st, lmap->data.as<int32_t>(), lmap->size, false, scols));
     if (!rmap || (pruned && build_out.empty())) return left.release();
     TableRef right(gather_table(build_table.t, rmap->data.as<int32_t>(), rmap->size, kind == B2_JOIN_LEFT_OUTER || kind == B2_JOIN_FULL_OUTER,
                                 pruned ? &build_out : nullptr));
@@ -976,7 +966,7 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
   bool sp_active = false, sp_read = false;
   struct Bucket {
     std::vector<SpillPiece> build, stream;
-    int64_t build_bytes = 0, stream_bytes = 0;
+    int64_t build_bytes = 0;
     bool resplit = false;   // made by repartitioning a bucket: never split again
   };
   std::deque<Bucket> sp_buckets;
@@ -1004,7 +994,7 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
                   BucketOf&& bucket_of, bool build_side, int64_t* bytes_out) {
     split_pieces(t, d_sel, n, keys, keep, seed, nparts, [&](int p, SpillPiece&& s) {
       Bucket& b = bucket_of(p);
-      (build_side ? b.build_bytes : b.stream_bytes) += s.bytes;
+      if (build_side) b.build_bytes += s.bytes;
       if (bytes_out) *bytes_out += s.bytes;
       (build_side ? b.build : b.stream).push_back(std::move(s));
     });
@@ -1061,7 +1051,7 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
       split_into(raw.t, sel.c ? sel.c->data.as<int32_t>() : nullptr, sel.c ? sel.c->size : raw.t->rows, keys, keep, SP_SEED, sp_parts,
                  first_level, false, &sp_stats[3]);
     }
-    if (!stream_schema.t && (coalesced() || tracked()))
+    if (!stream_schema.t && tracked())
       throw Error(B2_ERR_UNSUPPORTED, "empty stream side of an outer join that preserves the build side needs the stream schema");
   }
   bool useless(const Bucket& b) const {
@@ -1070,14 +1060,12 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
     if (kind == B2_JOIN_RIGHT_OUTER) return b.build.empty();   // build rows without stream rows are still output
     return b.stream.empty();   // LEFT OUTER / ANTI: stream rows without build rows are still output
   }
-  // GpuSubPartitionPairIterator: a bucket still over the target is split once more, with its stream pieces.  FULL OUTER without
-  // a condition coalesces a pair's stream side, so there a bucket whose stream pieces pass the target is split again as well.
+  // GpuSubPartitionPairIterator: a bucket whose build pieces are still over the target is split once more, with its stream pieces
   void repartition() {
     Bucket b = std::move(sp_buckets.front());
     sp_buckets.pop_front();
     sp_stats[1]++;
-    const int64_t bytes = std::max(b.build_bytes, coalesced() ? b.stream_bytes : 0);
-    const int k2 = (int)std::min<int64_t>(256, std::max<int64_t>(sp_parts, bytes / sp_target + 1));
+    const int k2 = (int)std::min<int64_t>(256, std::max<int64_t>(sp_parts, b.build_bytes / sp_target + 1));
     std::vector<Bucket> sub(k2);
     auto second_level = [&](int p) -> Bucket& { return sub[p]; };
     std::vector<int> all_b, all_s;
@@ -1088,32 +1076,27 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
     for (int p = k2 - 1; p >= 0; p--) { sub[p].resplit = true; sp_buckets.push_front(std::move(sub[p])); }
   }
   // GpuBatchSubPartitionIterator: the next pair = adjacent useful buckets whose build pieces together stay within the target.
-  // Builds its hash table (and tracker) and queues its stream pieces in probe groups of at most the target (FULL OUTER without a
-  // condition: one group).
+  // Builds its hash table (and tracker) and queues its stream pieces in probe groups of at most the target.
   bool open_next_pair() {
     if (tracker) { b2_join_tracker_close(tracker); tracker = 0; }
     if (ht) { b2_join_hash_table_close(ht); ht = 0; }
     build_table.reset();
-    auto over = [&](const Bucket& b) {
-      return !b.resplit && (b.build_bytes > sp_target || (coalesced() && b.stream_bytes > sp_target));
-    };
+    auto over = [&](const Bucket& b) { return !b.resplit && b.build_bytes > sp_target; };
     while (!sp_buckets.empty()) {
       if (useless(sp_buckets.front())) sp_buckets.pop_front();
       else if (over(sp_buckets.front())) repartition();
       else break;
     }
     if (sp_buckets.empty()) return false;
-    // FULL OUTER without a condition coalesces the pair's stream side as well, so its stream pieces count against the target too
-    const bool full = coalesced();
     std::vector<Bucket> pair;
-    int64_t bytes = sp_buckets.front().build_bytes, sbytes = sp_buckets.front().stream_bytes;
+    int64_t bytes = sp_buckets.front().build_bytes;
     pair.push_back(std::move(sp_buckets.front()));
     sp_buckets.pop_front();
     while (!sp_buckets.empty()) {
       const Bucket& nb = sp_buckets.front();
       if (useless(nb)) { sp_buckets.pop_front(); continue; }
-      if (over(nb) || bytes + nb.build_bytes > sp_target || (full && sbytes + nb.stream_bytes > sp_target)) break;
-      bytes += nb.build_bytes; sbytes += nb.stream_bytes;
+      if (over(nb) || bytes + nb.build_bytes > sp_target) break;
+      bytes += nb.build_bytes;
       pair.push_back(std::move(sp_buckets.front()));
       sp_buckets.pop_front();
     }
@@ -1125,7 +1108,6 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
     build_table = TableRef(concat_pieces(bp, sp_build_empty.t));
     bp.clear();
     build_hash(true);
-    if (full) { sp_probe.push_back(std::move(sps)); return true; }
     std::vector<SpillPiece> grp;
     int64_t gb = 0, gr = 0;
     for (auto& p : sps) {

@@ -159,7 +159,7 @@ __device__ __forceinline__ uint64_t join_entry(const uint64_t* __restrict__ slot
   return slots[idx];
 }
 
-// Matched build rows across stream batches (RIGHT OUTER, and FULL OUTER with a condition): a JoinTracker holds one bit per build
+// Matched build rows across stream batches (RIGHT OUTER and FULL OUTER): a JoinTracker holds one bit per build
 // row of one hash table, and the tracking (TRACK) probe variants set bit br where they find build row br — inside the probe,
 // where the reference filters the gather map, copies it, scatters it into a BOOL8 tracker and rebuilds the tracker per batch
 // (HashJoinStreamSideIterator.updateTrackingMask, GpuHashJoin.scala:2164-2204).  The word is read first and the atomic issued

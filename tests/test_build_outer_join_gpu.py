@@ -1,6 +1,6 @@
 """Outer joins that preserve the build side: JOIN_RIGHT_OUTER through every probe path of join.cu, the JoinTracker across
-probe batches, and GpuShuffledHashJoinExec with RIGHT OUTER (and FULL OUTER with a condition) over batches, filters,
-pruning, memory limits and sub-partitioning, against exact references.
+probe batches, and GpuShuffledHashJoinExec with RIGHT OUTER and FULL OUTER (with and without a condition) over batches,
+filters, pruning, memory limits and sub-partitioning, against exact references.
 
 RIGHT OUTER's reference maps are the FULL OUTER rows of join_maps that carry a build row: the inner pairs, then
 (INT32_MIN, b) for every build row b no probe row matched.  Each primitive probe asserts from the kernel timings which
@@ -301,7 +301,8 @@ def run_exec(b2, sides, kind, filt, prune, nulls_equal, cond, target=None, npart
 
 @pytest.mark.parametrize("prune", [False, True], ids=["all_columns", "pruned"])
 @pytest.mark.parametrize("filt", ["none", "simple", "like"])
-@pytest.mark.parametrize("kind,cond", [(RIGHT_OUTER, False), (RIGHT_OUTER, True), (FULL_OUTER, True)], ids=["right", "right_cond", "full_cond"])
+@pytest.mark.parametrize("kind,cond", [(RIGHT_OUTER, False), (RIGHT_OUTER, True), (FULL_OUTER, False), (FULL_OUTER, True)],
+                         ids=["right", "right_cond", "full", "full_cond"])
 def test_exec(b2, kind, cond, filt, prune):
     """multi-batch stream (one batch empty, the filter passes no row of the last) and build sides (one with NULL keys)"""
     rng = np.random.default_rng(40 + kind + 2 * cond)
@@ -335,7 +336,7 @@ def test_exec_edges(b2):
     from spark_rapids_b200 import execs as E
     rng = np.random.default_rng(45)
     stream, build, sbatches, bbatches = _sides(rng)
-    for kind, cond in ((RIGHT_OUTER, None), (FULL_OUTER, b2.col(1, b2.INT32, nullable=False) >= b2.col(8, b2.INT32, nullable=False))):
+    for kind, cond in ((RIGHT_OUTER, None), (FULL_OUTER, None), (FULL_OUTER, b2.col(1, b2.INT32, nullable=False) >= b2.col(8, b2.INT32, nullable=False))):
         j = E.GpuShuffledHashJoinExec([0], [0], kind, E.GpuBatchSource([]), E.GpuBatchSource([to_table(b2, b) for b in bbatches]), condition=cond)
         with pytest.raises(b2.B2Error) as e:            # no stream batch at all: the stream schema is unknown
             j.collect()
@@ -356,8 +357,8 @@ def _host(cols, rows):
     return [[(O.INT64, 0, c[s:s + rows], None) for c in cols] for s in range(0, len(cols[0]), rows)]
 
 
-@pytest.mark.parametrize("kind", [RIGHT_OUTER, FULL_OUTER], ids=["right", "full_cond"])
-def test_beyond_the_allocation_limit(b2, limits, kind):
+@pytest.mark.parametrize("kind,cond", [(RIGHT_OUTER, False), (FULL_OUTER, False), (FULL_OUTER, True)], ids=["right", "full", "full_cond"])
+def test_beyond_the_allocation_limit(b2, limits, kind, cond):
     """an 8 MiB build side (2^18 rows of four INT64 columns: its hash table takes 8.25 MiB more) and a 96 MiB stream side in
     2 MiB host batches, 32 MiB above the base: finishes without sub-partitioning, one stream batch at a time"""
     from spark_rapids_b200 import execs as E
@@ -371,9 +372,9 @@ def test_beyond_the_allocation_limit(b2, limits, kind):
     b2.sync()
     base = b2.device_bytes_in_use()
     b2.set_alloc_limit(base + (32 << 20))
-    cond = b2.col(3, b2.INT64, nullable=False) >= b2.lit(nb // 8, b2.INT64) if kind == FULL_OUTER else None
+    condition = b2.col(3, b2.INT64, nullable=False) >= b2.lit(nb // 8, b2.INT64) if cond else None
     node = E.GpuShuffledHashJoinExec([0], [0], kind, E.GpuHostBatchSource(_host([sk, sp], rows)),
-                                     E.GpuHostBatchSource(_host([bk, bp, bp * 3, bp * 5], rows // 2)), condition=cond)
+                                     E.GpuHostBatchSource(_host([bk, bp, bp * 3, bp * 5], rows // 2)), condition=condition)
     gs, gb = [], []
     for t in node:
         s, b = t.column(1).to_numpy(), t.column(3).to_numpy()
@@ -384,7 +385,7 @@ def test_beyond_the_allocation_limit(b2, limits, kind):
     got_s, got_b = np.concatenate(gs), np.concatenate(gb)
     assert node.metrics["numOutputRows"] == len(got_s)
     il, ir = join_maps([ocol(bk, O.INT64)], [ocol(sk, O.INT64)], INNER)
-    if kind == FULL_OUTER:
+    if cond:
         ok = ir >= nb // 8
         il, ir = il[ok], ir[ok]
     hitb = np.zeros(nb, bool)
@@ -459,7 +460,8 @@ def test_final_batch_split(b2, limits):
 
 
 # ---- 5. sub-partitioning ------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("kind,cond", [(RIGHT_OUTER, False), (RIGHT_OUTER, True), (FULL_OUTER, True)], ids=["right", "right_cond", "full_cond"])
+@pytest.mark.parametrize("kind,cond", [(RIGHT_OUTER, False), (RIGHT_OUTER, True), (FULL_OUTER, False), (FULL_OUTER, True)],
+                         ids=["right", "right_cond", "full", "full_cond"])
 def test_sub_partitioned(b2, kind, cond):
     rng = np.random.default_rng(50 + kind + cond)
     sides = _sides(rng)

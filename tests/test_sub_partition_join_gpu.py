@@ -1,7 +1,7 @@
 """Join build sides larger than the target (GpuSubPartitionHashJoin): b2_hash_split against the murmur3 oracle, and the
 sub-partitioned GpuShuffledHashJoinExec against the exact join reference (join_maps) for every join kind, NULL-key rule,
-filter below the stream side, column pruning and non-equi condition, with forced repartitions, skew and a build side (and
-for FULL OUTER a stream side) larger than the allocation limit."""
+filter below the stream side, column pruning and non-equi condition, with forced repartitions, skew and a build side larger
+than the allocation limit; and a FULL OUTER stream side larger than that limit, with and without sub-partitioning."""
 import gc
 
 import numpy as np
@@ -307,7 +307,7 @@ def test_join_matrix(b2, kind, filtered, prune):
         for cond in ([False] if kind == FULL_OUTER else [False, True]):
             st = _run_join(b2, sides, kind, filtered, prune, nulls_equal, cond, bb // 5, 16)         # several packed buckets
             assert st["buckets"] == 16 and st["build_bytes"] > 0 and st["stream_bytes"] > 0, st
-            assert st["repartitioned"] == 0 or kind == FULL_OUTER, st      # FULL OUTER also splits a bucket whose stream side is over
+            assert st["repartitioned"] == 0, st
             st = _run_join(b2, sides, kind, filtered, prune, nulls_equal, cond, int(bb * 0.4), 2)     # each half is over: split again
             assert st["buckets"] == 2 and st["repartitioned"] >= 1, st
 
@@ -332,9 +332,7 @@ def test_below_target_is_the_default_join(b2, kind):
     bb = _build_bytes(b2, bbatches)
     res = []
     for target in (None, bb, bb * 4):
-        src = E.GpuBatchSource([to_table(b2, s) for s in sbatches])
-        if kind != FULL_OUTER:
-            src = E.GpuFilterExec(b2.col(1, b2.INT32, nullable=False) >= b2.lit(500, b2.INT32), src)
+        src = E.GpuFilterExec(b2.col(1, b2.INT32, nullable=False) >= b2.lit(500, b2.INT32), E.GpuBatchSource([to_table(b2, s) for s in sbatches]))
         kw = {} if target is None else dict(target_bytes=target)
         j = E.GpuShuffledHashJoinExec([0], [0], kind, src, E.GpuBatchSource([to_table(b2, b) for b in bbatches]), stream_out=[2, 0], build_out=[1], **kw)
         b2.profile_enable(True)
@@ -404,7 +402,8 @@ def _collect_pairs(node):
 
 @pytest.mark.parametrize("kind", [INNER, FULL_OUTER])
 def test_beyond_the_allocation_limit(b2, limits, kind):
-    """INNER: a 96 MiB build side; FULL OUTER: a 96 MiB stream side (8 MiB build side); the limit is 32 MiB above the base"""
+    """INNER: a 96 MiB build side, which does not fit without sub-partitioning; FULL OUTER: a 96 MiB stream side (8 MiB build
+    side), joined one stream batch at a time with or without it; the limit is 32 MiB above the base"""
     from spark_rapids_b200 import execs as E
     rng = np.random.default_rng(17)
     rows = 1 << 17                                           # 2 MiB batches of [INT64 key, INT64 payload]
@@ -417,23 +416,37 @@ def test_beyond_the_allocation_limit(b2, limits, kind):
     base = b2.device_bytes_in_use()
     spilled0 = b2.memory_stats()["spilled_bytes"]
     b2.set_alloc_limit(base + (32 << 20))
-    mk = lambda **kw: E.GpuShuffledHashJoinExec([0], [0], kind, E.GpuHostBatchSource(_host(sk, sp, rows)), E.GpuHostBatchSource(_host(bk, bp, rows)), **kw)
-    single = mk()
-    with pytest.raises(b2.B2Error) as ei:
-        single.collect()
-    assert ei.value.code == ERR_OOM
-    del single, ei
-    gc.collect()
-    b2.sync()
-    node = mk(target_bytes=4 << 20)
-    got_s, got_b = _collect_pairs(node)
-    assert b2.memory_stats()["spilled_bytes"] > spilled0
-    assert node.metrics["numOutputRows"] == len(got_s) and node.sub_partition_stats["buckets"] == 16
+    mk = lambda srows, **kw: E.GpuShuffledHashJoinExec([0], [0], kind, E.GpuHostBatchSource(_host(sk, sp, srows)), E.GpuHostBatchSource(_host(bk, bp, rows)), **kw)
     lm, rm = join_maps([ocol(bk, O.INT64)], [ocol(sk, O.INT64)], kind)
     ws = np.where(lm >= 0, sp[np.maximum(lm, 0)], -1)
     wb = np.where(rm >= 0, bp[np.maximum(rm, 0)], -1)
-    og, ow = np.lexsort((got_b, got_s)), np.lexsort((wb, ws))
-    assert np.array_equal(got_s[og], ws[ow]) and np.array_equal(got_b[og], wb[ow])
+    ow = np.lexsort((wb, ws))
+
+    def check(got_s, got_b):
+        og = np.lexsort((got_b, got_s))
+        assert np.array_equal(got_s[og], ws[ow]) and np.array_equal(got_b[og], wb[ow])
+
+    if kind == INNER:
+        single = mk(rows)
+        with pytest.raises(b2.B2Error) as ei:
+            single.collect()
+        assert ei.value.code == ERR_OOM
+        del ei
+    else:   # batch by batch: the whole output does not fit under the limit
+        # in 512 KiB stream batches: the build side and its hash table (16.5 MiB) take 24.5 MiB of the limit, and the source
+        # holds three stream batches while the previous output batch is still alive
+        single = mk(rows // 4)
+        got_s, got_b = _collect_pairs(single)
+        assert single.metrics["numOutputRows"] == len(got_s) and single.sub_partition_stats["buckets"] == 0
+        check(got_s, got_b)
+    del single
+    gc.collect()
+    b2.sync()
+    node = mk(rows, target_bytes=4 << 20)
+    got_s, got_b = _collect_pairs(node)
+    assert b2.memory_stats()["spilled_bytes"] > spilled0
+    assert node.metrics["numOutputRows"] == len(got_s) and node.sub_partition_stats["buckets"] == 16
+    check(got_s, got_b)
     del node
     gc.collect()
     b2.sync()
