@@ -22,6 +22,7 @@
 #include <chrono>
 #include <cmath>
 #include <deque>
+#include <numeric>
 #include "joinemit.cuh"
 #include "vm.cuh"
 #include "window.cuh"
@@ -46,8 +47,7 @@ std::vector<Table*> hash_split_table(const Table* t, const int32_t* d_sel, int64
 // RmmRapidsRetryIterator.withRetry (RmmRapidsRetryIterator.scala:65-203): an allocation failure first spills (core.cu does
 // that inside the allocator) and surfaces as B2_ERR_OOM = GpuRetryOOM; the operator then makes everything spillable leave
 // the device, waits for the stream and runs the attempt again.  After two retries the error is handed to the caller, which
-// for joins and aggregates splits the input batch in halves and retries each (GpuSplitAndRetryOOM semantics,
-// AbstractGpuJoinIterator.scala:235-250 for the join's 2^31 output limit).
+// may halve its work with split_and_retry.
 template <typename F>
 static auto with_retry(F&& attempt) -> decltype(attempt()) {
   for (int n = 0;; n++) {
@@ -62,6 +62,21 @@ static auto with_retry(F&& attempt) -> decltype(attempt()) {
   }
 }
 static bool splittable(const Error& e) { return e.code == B2_ERR_OOM || e.code == B2_ERR_SIZE_OVERFLOW; }
+// GpuSplitAndRetryOOM (AbstractGpuJoinIterator.scala:235-250 for the join's 2^31 output limit): runs attempt(); when it fails
+// with B2_ERR_OOM (after its own retries) or B2_ERR_SIZE_OVERFLOW, split() replaces the work attempt() runs on with its two
+// halves, in row order, and attempt() runs again on the first half.  split() returns false when the work has fewer than 2
+// rows, and the error is handed on.  attempt() is not retried here: each caller runs with_retry around the steps inside it.
+template <typename A, typename S>
+static auto split_and_retry(A&& attempt, S&& split) -> decltype(attempt()) {
+  while (true) {
+    try {
+      return attempt();
+    } catch (const Error& e) {
+      if (!splittable(e) || !split()) throw;
+      note_split();
+    }
+  }
+}
 
 struct TableRef {  // owning reference
   Table* t = nullptr;
@@ -75,6 +90,20 @@ struct TableRef {  // owning reference
   void reset() { if (t) table_release(t); t = nullptr; }
   Table* release() { Table* r = t; t = nullptr; return r; }
 };
+
+// split() of split_and_retry over batches waiting in q, front first: the front batch is replaced by its halves.  slice_table
+// copies, so at its peak the split holds the batch and both halves.
+static bool split_front(std::deque<TableRef>& q) {
+  const Table* t = q.front().t;
+  if (t->rows < 2) return false;
+  const int64_t mid = t->rows / 2;
+  TableRef lo(with_retry([&] { return slice_table(t, 0, mid); }));
+  TableRef hi(with_retry([&] { return slice_table(t, mid, t->rows); }));
+  q.pop_front();
+  q.push_front(std::move(hi));
+  q.push_front(std::move(lo));
+  return true;
+}
 
 static Table* from_handle_owned(b2_handle h) { return h ? reinterpret_cast<Table*>((intptr_t)h) : nullptr; }
 // raises the error of a failed b2_* call
@@ -103,6 +132,16 @@ static Table* null_rows(const Table* schema, int64_t n, const std::vector<int>* 
   if (n) CUDA_CHECK(cudaMemsetAsync(oob.c->data.p, 0x80, (size_t)n * 4, stream()));   // 0x80808080 < 0: out of bounds -> NULL row
   return gather_table(schema, oob.c->data.as<int32_t>(), n, true, cols);
 }
+// the columns idx of t, by reference
+static Table* columns_of(const Table* t, const std::vector<int>& idx) {
+  ColsGuard cols;
+  for (int i : idx) {
+    if (i < 0 || i >= (int)t->cols.size()) throw Error(B2_ERR_INVALID, "column index out of range");
+    col_incref(t->cols[i]);
+    cols.v.push_back(t->cols[i]);
+  }
+  return new_table(cols.release());
+}
 
 // A batch waiting in the spill store, with the facts about it that planning needs, so that planning never brings it back
 struct SpillPiece {
@@ -129,6 +168,12 @@ struct SpillPiece {
     b2_handle h = 0;
     ok(b2_spillable_get(sp, &h));
     return from_handle_owned(h);
+  }
+  // the batch back on the device, and the piece closed
+  Table* take() {
+    Table* t = with_retry([&] { return get(); });
+    close();
+    return t;
   }
 };
 
@@ -434,9 +479,9 @@ struct GpuHashAggregateExec : GpuExec {
   Table* without_counts(Table* t) {
     if (mode == B2_AGG_MODE_PARTIAL || counted.empty()) return t;
     TableRef in(t);
-    std::vector<Column*> cols(t->cols.begin(), t->cols.begin() + keys.size() + aggs.size());
-    for (Column* c : cols) col_incref(c);
-    return new_table(std::move(cols));
+    std::vector<int> cols(keys.size() + aggs.size());
+    std::iota(cols.begin(), cols.end(), 0);
+    return columns_of(t, cols);
   }
   // keys are the leading columns, then the aggregates, then the counts; keep_counts: an intermediate merge, whose result is
   // merged again, keeps the counts in every mode
@@ -479,22 +524,20 @@ struct GpuHashAggregateExec : GpuExec {
              r.t->cols[nk + na + nc + q]->data.as<int8_t>(), r.t->rows);
       s->null_count = -1;
     }
-    std::vector<Column*> out(r.t->cols.begin(), r.t->cols.begin() + nk + na + (mode == B2_AGG_MODE_PARTIAL || keep_counts ? nc : 0));
-    for (Column* c : out) col_incref(c);
-    return new_table(std::move(out));
+    cols.resize(nk + na + (mode == B2_AGG_MODE_PARTIAL || keep_counts ? nc : 0));
+    return columns_of(r.t, cols);
   }
-  // first-pass aggregation of one input batch; when the device cannot hold it the batch is split in halves, each half
-  // yields its own partial (the merge pass combines them like any other pair of partials)
-  void first_pass(const Table* in, std::vector<TableRef>& partials, int depth) {
-    try {
-      const std::vector<b2_agg_spec> u = update_specs();
-      partials.emplace_back(with_retry([&] { return scan_aggregate(program, has_pred, in, keys.data(), (int)keys.size(), u.data(), (int)u.size()); }));
-    } catch (const Error& e) {
-      if (!splittable(e) || in->rows < 2 || depth >= 12) throw;
-      note_split();
-      const int64_t mid = in->rows / 2;
-      { TableRef lo(slice_table(in, 0, mid)); first_pass(lo.t, partials, depth + 1); }
-      { TableRef hi(slice_table(in, mid, in->rows)); first_pass(hi.t, partials, depth + 1); }
+  // first-pass aggregation of one input batch (which it takes); when the device cannot hold it the batch is split in halves,
+  // each half yields its own partial (the merge pass combines them like any other pair of partials)
+  void first_pass(TableRef in, std::vector<TableRef>& partials) {
+    const std::vector<b2_agg_spec> u = update_specs();
+    std::deque<TableRef> work;
+    work.push_back(std::move(in));
+    while (!work.empty()) {
+      partials.emplace_back(split_and_retry(
+          [&] { return with_retry([&] { return scan_aggregate(program, has_pred, work.front().t, keys.data(), (int)keys.size(), u.data(), (int)u.size()); }); },
+          [&] { return split_front(work); }));
+      work.pop_front();
     }
   }
   Table* do_next() override {
@@ -506,7 +549,7 @@ struct GpuHashAggregateExec : GpuExec {
       TableRef in(children[0]->next());
       if (!in.t) break;
       if (mode == B2_AGG_MODE_FINAL) partials.emplace_back(in.release());   // inputs already are aggregation buffers
-      else first_pass(in.t, partials, 0);
+      else first_pass(std::move(in), partials);
     }
     return merge_all(partials);
   }
@@ -586,8 +629,7 @@ struct GpuHashAggregateExec : GpuExec {
       if (!in.t) break;
       if (mode == B2_AGG_MODE_FINAL) { take(std::move(in)); continue; }
       std::vector<TableRef> ps;
-      first_pass(in.t, ps, 0);
-      in.reset();
+      first_pass(std::move(in), ps);
       for (auto& p : ps) take(std::move(p));
     }
     if (bucketed) return true;
@@ -603,8 +645,7 @@ struct GpuHashAggregateExec : GpuExec {
     std::vector<AggBucket> sub(rp_parts);
     auto next_level = [&](int p) -> AggBucket& { return sub[p]; };
     for (auto& p : b.pieces) {
-      TableRef t(with_retry([&] { return p.get(); }));
-      p.close();
+      TableRef t(p.take());
       rp_split(t.t, depth, next_level);
     }
     for (int p = rp_parts - 1; p >= 0; p--) { sub[p].depth = depth; rp_buckets.push_front(std::move(sub[p])); }
@@ -676,7 +717,7 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
   // with_retry)
   void build_hash(bool retry) {
     auto make = [&] {
-      TableRef bk(select(build_table.t, build_keys));
+      TableRef bk(columns_of(build_table.t, build_keys));
       b2_handle h = 0;
       ok(b2_join_build(to_handle(bk.t), nulls_equal, &h));
       return h;
@@ -692,11 +733,6 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
     const b2_handle kh = to_handle(const_cast<Table*>(keys)), sh = sel ? to_handle(sel) : 0;
     if (!tracked()) { ok(b2_join_probe_sel(ht, kh, sh, kind, lm, rm)); return; }
     ok(b2_join_probe_track(ht, kh, sh, kind == B2_JOIN_FULL_OUTER ? B2_JOIN_LEFT_OUTER : B2_JOIN_INNER, tracker, lm, rm));
-  }
-  static Table* select(const Table* t, const std::vector<int>& idx) {
-    std::vector<Column*> cols;
-    for (int i : idx) { if (i < 0 || i >= (int)t->cols.size()) throw Error(B2_ERR_INVALID, "join key index out of range"); col_incref(t->cols[i]); cols.push_back(t->cols[i]); }
-    return new_table(std::move(cols));
   }
   void build() {
     // prepareBuildBatchesForJoin: the whole build side becomes one batch
@@ -760,7 +796,7 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
       for (int k : stream_keys) f_keys.push_back(fused->input_col(k));
       if (pruned) for (int c : stream_out) f_stream.push_back(fused->input_col(c));
       else f_stream = f_all;
-      if (tracked()) { TableRef cols(select(raw.t, f_all)); stream_schema = TableRef(slice_table(cols.t, 0, 0)); }
+      if (tracked()) { TableRef cols(columns_of(raw.t, f_all)); stream_schema = TableRef(slice_table(cols.t, 0, 0)); }
     }
     // simple predicate + FK -> PK inner probe: the filter is evaluated INSIDE the probe kernel (no selection vector at all)
     struct Owned { Column* c = nullptr; ~Owned() { if (c) col_release(c); } Column* take() { Column* r = c; c = nullptr; return r; } };
@@ -785,7 +821,7 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
         if (plm.c) { lmc = plm.take(); rmc = prm.take(); }   // the maps of the fused kernel (first attempt only)
         else {
           make_sel();
-          TableRef sk(select(raw.t, f_keys));
+          TableRef sk(columns_of(raw.t, f_keys));
           b2_handle lm = 0, rm = 0;
           probe(sk.t, sel.c, &lm, &rm);
           lmc = col_from(lm); rmc = rm ? col_from(rm) : nullptr;
@@ -802,7 +838,7 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
       // memory pressure / 2^31 limit: materialise the filter output after all and take the split-and-retry path
       make_sel();
       TableRef ft(gather_table(raw.t, sel.c->data.as<int32_t>(), sel.c->size, false, &f_all));
-      todo.emplace_back(std::move(ft), 0);
+      todo.push_back(std::move(ft));
       return drain_todo();
     }
   }
@@ -818,7 +854,7 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
     TableRef s(children[0]->next());
     if (!s.t) return tracked() ? final_start() : nullptr;
     if (tracked() && !stream_schema.t) stream_schema = TableRef(slice_table(s.t, 0, 0));
-    todo.emplace_back(std::move(s), 0);
+    todo.push_back(std::move(s));
     return drain_todo();
   }
   // Tracked joins, after the last stream batch (of the pair, when sub-partitioned): the build rows never marked, NULL on the
@@ -838,19 +874,17 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
     return fin.empty() ? nullptr : final_next();
   }
   Table* final_next() {
-    while (true) {
+    Table* out = split_and_retry([&] { return with_retry([&] { return final_rows(fin.front().first, fin.front().second); }); }, [&] {
       const std::pair<int64_t, int64_t> r = fin.front();
+      if (r.second - r.first < 2) return false;
+      const int64_t mid = r.first + (r.second - r.first) / 2;
       fin.pop_front();
-      try {
-        return with_retry([&] { return final_rows(r.first, r.second); });
-      } catch (const Error& e) {
-        if (!splittable(e) || r.second - r.first < 2) throw;
-        note_split();
-        const int64_t mid = r.first + (r.second - r.first) / 2;
-        fin.emplace_front(mid, r.second);
-        fin.emplace_front(r.first, mid);
-      }
-    }
+      fin.emplace_front(mid, r.second);
+      fin.emplace_front(r.first, mid);
+      return true;
+    });
+    fin.pop_front();
+    return out;
   }
   Table* final_rows(int64_t lo, int64_t hi) {
     const int64_t n = hi - lo;
@@ -859,31 +893,15 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
     return concat_cols(left.t, right.t);
   }
   // stream slices waiting to be joined (a batch that had to be split leaves its halves here; one output per next())
-  std::deque<std::pair<TableRef, int>> todo;
-  // one stream batch -> output batch(es).  When the gather maps would pass 2^31-1 rows (B2_ERR_SIZE_OVERFLOW) or the device
-  // cannot hold the output (B2_ERR_OOM after retries) the stream batch is halved and each half joined on its own — lazily,
-  // so that at most one output batch exists at a time (GpuSplitAndRetryOOM, AbstractGpuJoinIterator.scala:235-250)
+  std::deque<TableRef> todo;
+  // the front stream batch -> one output batch.  When the gather maps would pass 2^31-1 rows (B2_ERR_SIZE_OVERFLOW) or the
+  // device cannot hold the output (B2_ERR_OOM after retries) the stream batch is halved and each half joined on its own —
+  // lazily, so that at most one output batch exists at a time
   Table* drain_todo() {
-    while (!todo.empty()) {
-      TableRef st = std::move(todo.front().first);
-      const int depth = todo.front().second;
-      todo.pop_front();
-      try {
-        Table* out = with_retry([&] { return join_batch(st.t); });
-        em_stats[1]++;
-        return out;
-      } catch (const Error& e) {
-        if (!splittable(e) || st.t->rows < 2 || depth >= 16) throw;
-        note_split();
-        const int64_t mid = st.t->rows / 2;
-        // the halves replace the batch: the batch itself is released before they are made, so the split needs no extra room
-        TableRef lo(slice_table(st.t, 0, mid)), hi(slice_table(st.t, mid, st.t->rows));
-        st.reset();
-        todo.emplace_front(std::move(hi), depth + 1);
-        todo.emplace_front(std::move(lo), depth + 1);
-      }
-    }
-    return nullptr;
+    Table* out = split_and_retry([&] { return with_retry([&] { return join_batch(todo.front().t); }); }, [&] { return split_front(todo); });
+    todo.pop_front();
+    em_stats[1]++;
+    return out;
   }
   // the output rows of stream batch `st` (its columns `scols`; null: all) from the gather maps: stream columns ++ build columns
   // (GpuHashJoin.scala:2451-2470).  Without a right map (semi / anti) or anything wanted from the build side: the stream columns.
@@ -895,16 +913,9 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
     if (pruned && stream_out.empty()) return right.release();
     return concat_cols(left.t, right.t);
   }
-  Table* prune_pairs(const Table* pairs, int nstream) {   // [stream ++ build] -> the output columns of the node
-    std::vector<Column*> cols;
-    auto take = [&](int i) { col_incref(pairs->cols[i]); cols.push_back(pairs->cols[i]); };
-    if (pruned) { for (int c : stream_out) take(c); for (int c : build_out) take(nstream + c); }
-    else for (int i = 0; i < (int)pairs->cols.size(); i++) take(i);
-    return new_table(std::move(cols));
-  }
   // equi-join pairs -> condition over the pair rows -> per join type
   Table* join_batch_conditional(const Table* st) {
-    TableRef sk(select(st, stream_keys));
+    TableRef sk(columns_of(st, stream_keys));
     b2_handle lm = 0, rm = 0;
     ok(b2_join_probe(ht, to_handle(sk.t), B2_JOIN_INNER, &lm, &rm));
     ColGuard lmap(col_from(lm)), rmap(col_from(rm));
@@ -919,36 +930,40 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
     if (pass->dtype != B2_BOOL8) throw Error(B2_ERR_INVALID, "join condition must be BOOL8");
     // the build rows of the pairs that pass (marking is idempotent: a retried or halved batch sets the same bits)
     if (tracker) ok(b2_join_tracker_mark(tracker, to_handle(rmap.c), to_handle(pass)));
-    auto stream_side = [&](const Table* t) {   // semi / anti output: the node's stream columns
-      std::vector<Column*> cols;
-      if (pruned) for (int c : stream_out) { col_incref(t->cols[c]); cols.push_back(t->cols[c]); }
-      else for (auto* c : t->cols) { col_incref(c); cols.push_back(c); }
-      return new_table(std::move(cols));
-    };
+    // the output columns of the node among the pair columns [stream ++ build], and its stream columns (the semi / anti output)
+    std::vector<int> out_cols, stream_cols;
+    if (pruned) {
+      stream_cols = out_cols = stream_out;
+      for (int c : build_out) out_cols.push_back(nstream + c);
+    } else {
+      out_cols.resize(pairs.t->cols.size());
+      std::iota(out_cols.begin(), out_cols.end(), 0);
+      stream_cols.assign(out_cols.begin(), out_cols.begin() + nstream);
+    }
     if (kind == B2_JOIN_INNER || kind == B2_JOIN_RIGHT_OUTER) {
-      TableRef out(prune_pairs(pairs.t, nstream));
+      TableRef out(columns_of(pairs.t, out_cols));
       return filter_by_mask(out.t, pass);
     }
     if (kind == B2_JOIN_LEFT_SEMI || kind == B2_JOIN_LEFT_ANTI) {
       ColGuard flags(rows_with_passing_pair(lmap.c, pass, st->rows, kind == B2_JOIN_LEFT_ANTI));
-      TableRef side(stream_side(st));
+      TableRef side(columns_of(st, stream_cols));
       return filter_by_mask(side.t, flags.c);
     }
     // LEFT OUTER (and FULL OUTER's per-batch part): the passing pairs, then every stream row without one, NULL on the build side
-    TableRef pruned_pairs(prune_pairs(pairs.t, nstream));
+    TableRef pruned_pairs(columns_of(pairs.t, out_cols));
     TableRef matched(filter_by_mask(pruned_pairs.t, pass));
     ColGuard lonely(rows_with_passing_pair(lmap.c, pass, st->rows, true));
     TableRef lonely_stream(filter_by_mask(st, lonely.c));
     TableRef nulls(null_rows(build_table.t, lonely_stream.t->rows, nullptr));
     TableRef lonely_pairs(concat_cols(lonely_stream.t, nulls.t));
-    TableRef lonely_out(prune_pairs(lonely_pairs.t, nstream));
+    TableRef lonely_out(columns_of(lonely_pairs.t, out_cols));
     // nullability must agree for the concatenation: concat_tables merges validity
     std::vector<const Table*> ts{matched.t, lonely_out.t};
     return concat_tables(ts);
   }
   Table* join_batch(const Table* st) {
     if (condition) return join_batch_conditional(st);
-    TableRef sk(select(st, stream_keys));
+    TableRef sk(columns_of(st, stream_keys));
     b2_handle lm = 0, rm = 0;
     probe(sk.t, nullptr, &lm, &rm);
     ColGuard lmap(col_from(lm));
@@ -1019,11 +1034,10 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
       sp_buckets.resize(sp_parts);
       sp_bkeys = build_keys;
       sp_bkeep = carried((int)b.t->cols.size(), build_keys, build_out);
-      { TableRef sel(select(b.t, sp_bkeep)); sp_build_empty = TableRef(slice_table(sel.t, 0, 0)); }
+      { TableRef sel(columns_of(b.t, sp_bkeep)); sp_build_empty = TableRef(slice_table(sel.t, 0, 0)); }
       b.reset();
       for (auto& h : held) {
-        TableRef t(with_retry([&] { return h.get(); }));
-        h.close();
+        TableRef t(h.take());
         split(t.t);
       }
       held.clear();
@@ -1044,7 +1058,7 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
         auto raw_of = [&](int c) { return fused ? fused->input_col(c) : c; };
         for (int k : stream_keys) keys.push_back(raw_of(k));
         for (int c : carried(ncols, stream_keys, stream_out)) keep.push_back(raw_of(c));
-        TableRef sel(select(raw.t, keep));
+        TableRef sel(columns_of(raw.t, keep));
         stream_schema = TableRef(slice_table(sel.t, 0, 0));
       }
       ColGuard sel(fused ? fused->row_ids(raw.t) : nullptr);
@@ -1071,8 +1085,8 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
     std::vector<int> all_b, all_s;
     for (int c = 0; c < (int)sp_build_empty.t->cols.size(); c++) all_b.push_back(c);
     for (int c = 0; stream_schema.t && c < (int)stream_schema.t->cols.size(); c++) all_s.push_back(c);
-    for (auto& p : b.build) { TableRef t(with_retry([&] { return p.get(); })); p.close(); split_into(t.t, nullptr, t.t->rows, build_keys, all_b, SP_RESEED, k2, second_level, true, nullptr); }
-    for (auto& p : b.stream) { TableRef t(with_retry([&] { return p.get(); })); p.close(); split_into(t.t, nullptr, t.t->rows, stream_keys, all_s, SP_RESEED, k2, second_level, false, nullptr); }
+    for (auto& p : b.build) { TableRef t(p.take()); split_into(t.t, nullptr, t.t->rows, build_keys, all_b, SP_RESEED, k2, second_level, true, nullptr); }
+    for (auto& p : b.stream) { TableRef t(p.take()); split_into(t.t, nullptr, t.t->rows, stream_keys, all_s, SP_RESEED, k2, second_level, false, nullptr); }
     for (int p = k2 - 1; p >= 0; p--) { sub[p].resplit = true; sp_buckets.push_front(std::move(sub[p])); }
   }
   // GpuBatchSubPartitionIterator: the next pair = adjacent useful buckets whose build pieces together stay within the target.
@@ -1126,7 +1140,7 @@ struct GpuShuffledHashJoinExec : GpuExec {  // children[0] = stream (left), chil
       if (!sp_probe.empty()) {
         std::vector<SpillPiece> grp = std::move(sp_probe.front());
         sp_probe.pop_front();
-        todo.emplace_back(TableRef(concat_pieces(grp, stream_schema.t)), 0);
+        todo.emplace_back(concat_pieces(grp, stream_schema.t));
         continue;
       }
       if (ht && tracked() && !fin_started) {   // the pair's last group is done (or it had none): its unmatched build rows
@@ -1349,13 +1363,13 @@ struct GpuOutOfCoreSortExec : GpuExec {
     size_t n = 1;
     int64_t rows = final_q[0].rows;
     while (n < final_q.size() && rows + final_q[n].rows <= 0x7fffffffLL && output_bytes(n + 1) <= target) rows += final_q[n++].rows;
+    std::vector<int> data_cols(dtypes.size() - 1);   // without the ordinal
+    std::iota(data_cols.begin(), data_cols.end(), 0);
     Table* out = with_retry([&] {
       std::vector<TableRef> parts;
       for (size_t i = 0; i < n; i++) {
         TableRef t(final_q[i].get());
-        std::vector<Column*> cols(t.t->cols.begin(), t.t->cols.end() - 1);   // without the ordinal
-        for (Column* c : cols) col_incref(c);
-        parts.emplace_back(new_table(std::move(cols)));
+        parts.emplace_back(columns_of(t.t, data_cols));
       }
       return one_table(std::move(parts));
     });
@@ -1384,7 +1398,7 @@ struct GpuWindowExec : GpuExec {
   WindowPlan plan;
   WindowCarry carry;
   bool bound = false, done = false;
-  std::deque<TableRef> pending;   // mode 1: the later pieces of a split batch, in row order, run by the next calls
+  std::deque<TableRef> pending;   // mode 1: the batch to run and the later pieces of a split batch, in row order
   std::vector<SpillPiece> held;   // modes 2 and 3: rows of the group still open
   int64_t held_rows = 0;
   TableRef held_last;             // the last held row
@@ -1396,19 +1410,13 @@ struct GpuWindowExec : GpuExec {
   int64_t waiting_rows = 0;
   SpillPiece context;
 
-  // mode 1: on an OOM the batch is halved; the first half runs now and the second waits in `pending` (the carry makes the halves
-  // equivalent to the whole, and each half leaves as its own output batch, so no concatenation is needed)
-  Table* run(const Table* t) {
-    try {
-      return with_retry([&] { return window_chunk(plan, t, &carry); });
-    } catch (const Error& e) {
-      if (plan.mode != 1 || !splittable(e) || t->rows < 2) throw;
-      note_split();
-      const int64_t h = t->rows / 2;
-      TableRef a(with_retry([&] { return slice_table(t, 0, h); }));
-      pending.emplace_front(with_retry([&] { return slice_table(t, h, t->rows); }));
-      return run(a.t);
-    }
+  // mode 1: the front of `pending`.  On an OOM it is halved; the first half runs now and the second waits (the carry makes the
+  // halves equivalent to the whole, and each half leaves as its own output batch, so no concatenation is needed)
+  Table* run() {
+    Table* out = split_and_retry([&] { return with_retry([&] { return window_chunk(plan, pending.front().t, &carry); }); },
+                                 [&] { return split_front(pending); });
+    pending.pop_front();
+    return out;
   }
   static void hold(std::vector<SpillPiece>& into, int64_t& rows, const Table* t) {
     if (rows + t->rows > 0x7fffffffLL) throw Error(B2_ERR_SIZE_OVERFLOW, "window: a partition of more than 2^31-1 rows");
@@ -1417,16 +1425,10 @@ struct GpuWindowExec : GpuExec {
     into.push_back(std::move(p));
     rows += t->rows;
   }
-  Table* flush(std::vector<SpillPiece>& pieces) {
+  Table* flush(std::vector<SpillPiece>& pieces) {   // modes 2 and 3: a group runs whole, it cannot be halved
     TableRef chunk(concat_pieces(pieces, nullptr));
     pieces.clear();
-    return run(chunk.t);
-  }
-  // the read columns of t, by reference
-  Table* read_view(const Table* t) const {
-    ColsGuard cols;
-    for (int c : read_cols) { col_incref(t->cols[c]); cols.v.push_back(t->cols[c]); }
-    return new_table(cols.release());
+    return with_retry([&] { return window_chunk(plan, chunk.t, &carry); });
   }
   // bounded: the front batch's output, its context, rows and look-ahead in one chunk
   Table* run_front() {
@@ -1434,11 +1436,11 @@ struct GpuWindowExec : GpuExec {
     const int64_t rows = whole.t->rows, ctx = context.sp ? context.rows : 0;
     std::vector<TableRef> parts;
     if (ctx) parts.emplace_back(context.get());
-    parts.emplace_back(read_view(whole.t));
+    parts.emplace_back(columns_of(whole.t, read_cols));
     int64_t need = plan.post, total = ctx + rows;
     for (size_t j = 1; j < waiting.size() && need > 0; j++) {
       TableRef b(waiting[j].get());
-      TableRef v(read_view(b.t));
+      TableRef v(columns_of(b.t, read_cols));
       const int64_t take = std::min(need, b.t->rows);
       parts.emplace_back(take == b.t->rows ? v.release() : with_retry([&] { return slice_table(v.t, 0, take); }));
       need -= take;
@@ -1473,24 +1475,20 @@ struct GpuWindowExec : GpuExec {
   }
   // bounded: an OOM halves the front batch; the halves wait in its place and leave as two output batches
   Table* run_bounded() {
-    while (true) {
-      try {
-        return run_front();
-      } catch (const Error& e) {
-        if (!splittable(e) || waiting.front().rows < 2) throw;
-        note_split();
-        TableRef whole(waiting.front().get());
-        const int64_t n = whole.t->rows, h = n / 2;
-        TableRef a(with_retry([&] { return slice_table(whole.t, 0, h); }));
-        TableRef b(with_retry([&] { return slice_table(whole.t, h, n); }));
-        SpillPiece pa, pb;
-        pa.hold(a.t);
-        pb.hold(b.t);
-        waiting.pop_front();
-        waiting.push_front(std::move(pb));
-        waiting.push_front(std::move(pa));
-      }
-    }
+    return split_and_retry([&] { return run_front(); }, [&] {
+      if (waiting.front().rows < 2) return false;
+      TableRef whole(waiting.front().get());
+      const int64_t n = whole.t->rows, h = n / 2;
+      TableRef a(with_retry([&] { return slice_table(whole.t, 0, h); }));
+      TableRef b(with_retry([&] { return slice_table(whole.t, h, n); }));
+      SpillPiece pa, pb;
+      pa.hold(a.t);
+      pb.hold(b.t);
+      waiting.pop_front();
+      waiting.push_front(std::move(pb));
+      waiting.push_front(std::move(pa));
+      return true;
+    });
   }
   Table* next_bounded() {
     while (true) {
@@ -1508,11 +1506,7 @@ struct GpuWindowExec : GpuExec {
   }
   Table* do_next() override {
     if (plan.bounded) return next_bounded();
-    if (!pending.empty()) {
-      TableRef t(std::move(pending.front()));
-      pending.pop_front();
-      return run(t.t);
-    }
+    if (!pending.empty()) return run();
     while (true) {
       if (done) return nullptr;
       TableRef in(children[0]->next());
@@ -1523,7 +1517,10 @@ struct GpuWindowExec : GpuExec {
       }
       if (in.t->rows == 0) continue;
       if (!bound) { bind_window(plan, in.t); bound = true; }
-      if (plan.mode == 1) return run(in.t);
+      if (plan.mode == 1) {
+        pending.push_back(std::move(in));
+        return run();
+      }
       const int64_t n = in.t->rows;
       const int64_t start = with_retry([&] { return window_last_start(plan, in.t, held_last.t, plan.mode == 3 ? 1 : 2); });
       TableRef last(slice_table(in.t, n - 1, n));

@@ -1,5 +1,6 @@
 """(f4) memory-pressure contract and the threading contract of the boundary (SURVEY §8b): retryable OOM, spill store,
 split-and-retry in the join / aggregate execs, GpuSemaphore, re-entrancy from several host threads."""
+import gc
 import threading
 
 import numpy as np
@@ -109,6 +110,43 @@ def test_join_exec_splits_and_retries_under_memory_pressure(b2, limits):
     s1 = b2.memory_stats()
     assert s1["splits"] > s0["splits"] and nout >= 2, (s0, s1, nout)
     assert sorted(got) == exp
+
+
+def test_aggregate_splits_a_batch_under_memory_pressure(b2, limits):
+    """COMPLETE-mode SUM and COUNT by an INT64 key over one batch of n = 2^22 rows (16 B per row), each key about four times.
+    A first pass over more than 2^20 rows takes scan_aggregate's radix path: two row arrays of 20 B per row (hash, key, value),
+    28 B per row of group slots (key, two accumulator words, validity word), about 1 B per row of tile counts, 24 B per group
+    of output and the 2.25 MiB table of the cardinality probe.  Above what is in use with the batch, in B per row of the batch:
+    the whole batch's first pass needs about 77; the split, both halves beside the batch, 16; each half's first pass, with the
+    two halves (or one half and a partial) in place of the batch, about 36 + 5; the merge of the two partials (about 0.43 n
+    rows), once the batch is gone, about 31.  A limit of 60 forces one split, and the halves' partials merge to the whole's
+    result."""
+    from spark_rapids_b200 import execs as E
+    n = 1 << 22
+    rng = np.random.default_rng(12)
+    keys, vals = rng.integers(0, n // 4, n), rng.integers(-10**9, 10**9, n)
+    src = E.GpuBatchSource([b2.Table.from_columns([b2.Column.from_numpy(keys), b2.Column.from_numpy(vals)])])
+    pre = [b2.col(0, b2.INT64, nullable=False), b2.col(1, b2.INT64, nullable=False)]
+    specs = [(b2.AGG_SUM, 1, b2.INT64, 0, 0), (b2.AGG_COUNT_ALL, 0)]
+    node = E.GpuHashAggregateExec(src, [0], specs, pre_project=pre, mode="complete")
+    del src
+    gc.collect()
+    b2.sync()
+    s0 = b2.memory_stats()
+    b2.set_alloc_limit(b2.device_bytes_in_use() + 60 * n)
+    out = node.next()
+    b2.set_alloc_limit(0)
+    assert node.next() is None
+    s1 = b2.memory_stats()
+    assert s1["splits"] > s0["splits"], (s0, s1)
+    order = np.argsort(keys, kind="stable")
+    sk = keys[order]
+    starts = np.flatnonzero(np.r_[True, sk[1:] != sk[:-1]])
+    k, s, c = (out.column(i).to_numpy()[0] for i in range(3))
+    o = np.argsort(k)
+    assert np.array_equal(k[o], sk[starts])
+    assert np.array_equal(s[o], np.add.reduceat(vals[order], starts))
+    assert np.array_equal(c[o], np.diff(np.r_[starts, n]))
 
 
 def test_semaphore_bounds_concurrent_tasks(b2, limits):
